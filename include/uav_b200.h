@@ -85,23 +85,7 @@ typedef struct {
    * epilogue (n_out >= 33, aligned) and no GEGLU.  Deterministic (no atomics). */
   void* gn_partial;
   int64_t gn_blocks;
-  /* nn.LayerNorm folded into the Linear that consumes it (attention.py:525-563: norm1/2/temporal/3 -> to_q / q|k|v / GEGLU):
-   * the GEMM runs on the RAW rows x (K = normalised width) against W' = W * gamma (caller-packed), and the epilogue applies
-   *   LN(x) W^T + b  =  rstd[row] * (acc - mean[row] * colsum(W')[n]) + b'[n],     b' = b + W beta (passed as `bias`)
-   * so the normalised tensor is never written or read.  mean / rstd come from ln_in: fp32 [M][ln_slots][2] = partial
-   * {sum, sum of squares} of each input row, written by the Linear that PRODUCED x through ln_out (one slot per
-   * column half of each of its N-tiles — N-tiles are 128 columns wide when N > 64, else 64 — so ln_out_slots must equal
-   * uav_ln_partial_slots(N) of that launch).  Linear only. */
-  const void* ln_in;
-  const float* ln_colsum; /* fp32 [N]: sum over k of the fp16 W'[n][k] */
-  int ln_slots;
-  float ln_eps;
-  void* ln_out;
-  int ln_out_slots;
 } uav_epilogue_t;
-
-/* slots per row a Linear with n_out output columns writes through ln_out */
-int uav_ln_partial_slots(int64_t n_out);
 
 /* number of 16-row statistics blocks the implicit-GEMM launch over `images` images of `w` x `h` output pixels
  * produces (8 per M-tile; an M-tile is a tw x th = 128 pixel rectangle of one image, or 128 rows when h == 1) */
@@ -328,13 +312,12 @@ uav_status_t uav_add_noise(const void* x, const void* noise, void* out, int64_t 
                            uav_stream_t stream);
 /* one frame update of Propagation.forward, learnable=False (propagation_module.py:234-254):
  * fbConsistencyCheck mask + flow_warp(nearest|bilinear) + fuse + select, for C planes of H x W.
- * cs_* = channel (plane) strides in elements.  half_grid_sample: see csrc/sampler.cu. */
+ * cs_* = channel (plane) strides in elements. */
 uav_status_t uav_propagate_step(const void* feat_prop, const void* feat_cur, const void* flow_prop,
                                 const void* flow_check, void* out, int64_t C, int64_t H, int64_t W,
                                 int64_t cs_prop, int64_t cs_cur, int64_t cs_out,
                                 int64_t cs_flow_prop, int64_t cs_flow_check, int nearest, int fuse,
-                                float fuse_scale, float alpha1, float alpha2, int half_grid_sample,
-                                int dtype, uav_stream_t stream);
+                                float fuse_scale, float alpha1, float alpha2, int dtype, uav_stream_t stream);
 
 /* ---- after the decode: colour fix + output packing (SURVEY.md §8f rank 4) ---------------------------------
  * All tensors are the reference's planar fp32 "t c h w" frames (planes = t * c). */

@@ -35,17 +35,6 @@ def _epilogue(acc, bias, rowvec, rows_per_vec, residual, act, out, out_dtype, ou
     return v
 
 
-GN_FUSED_STATS = True  # mirrors ops.GN_FUSED_STATS (read by layers.new_cat_slot)
-LN_FUSED = False       # mirrors ops.LN_FUSED (read by layers._ln_linear); the folded path has its own test (it is slow to emulate)
-
-
-class EmuLn:
-    """stand-in for ops.LnStats: marks a token tensor whose producer emitted LayerNorm row statistics"""
-
-    def __init__(self, C):
-        self.C = C
-
-
 class EmuStats:
     """stand-in for ops.GnStats: marks a tensor whose producer "emitted" GroupNorm statistics, so that the host logic
     around them (virtual concat, slot allocation) runs on the CPU; the emulated GroupNorm recomputes its statistics"""
@@ -82,21 +71,10 @@ def group_norm_cat(parts, gamma, beta, groups, eps, *, silu, n_outer):
 
 
 def linear(a, w, bias=None, *, out=None, residual=None, rowvec=None, rows_per_vec=0, act=ACT_NONE, out_dtype=torch.float16,
-           out_scale=1.0, gn_stats=False, ln=None, ln_stats=False):
-    x = a.float().reshape(-1, a.shape[-1])
-    acc = x @ w.float().t()
-    if ln is not None:
-        # the kernel's folded LayerNorm: raw rows against W' = W * gamma, then rstd * (acc - mean * colsum(W')) (+ b' as bias)
-        _, colsum, eps = ln
-        mean = x.mean(dim=-1, keepdim=True)
-        var = (x * x).mean(dim=-1, keepdim=True) - mean * mean
-        rstd = torch.rsqrt(var.clamp(min=0) + eps)
-        acc = rstd * (acc - mean * colsum.float()[None, :])
+           out_scale=1.0, gn_stats=False):
+    acc = a.float().reshape(-1, a.shape[-1]) @ w.float().t()
     v = _epilogue(acc, bias, rowvec, rows_per_vec, residual, act, out, out_dtype, out_scale)
-    o = _finish(v, a.shape[:-1], out, out_dtype, gn_stats and act != ACT_GEGLU)
-    if ln_stats and act != ACT_GEGLU and o.dtype == torch.float16 and o.shape[-1] >= 64:
-        o.uav_ln = EmuLn(o.shape[-1])
-    return o
+    return _finish(v, a.shape[:-1], out, out_dtype, gn_stats and act != ACT_GEGLU)
 
 
 def _conv_nhwc(x4, w, stride, pads):

@@ -69,16 +69,6 @@ def test_unet_host_logic_vs_golden(emulated, unet_sd, case):
     assert not torch.equal(out, out3)
 
 
-def test_unet_host_logic_layernorm_folded(emulated, unet_sd, monkeypatch):
-    """opt-in path (UAV_LN_FUSED=1): every LayerNorm of the transformer blocks folded into the Linear that consumes it
-    (gamma-scaled weights, column sums, rank-1 correction) — same golden, same band"""
-    monkeypatch.setattr(emu_ops, "LN_FUSED", True)
-    c = torch.load(os.path.join(G, "unet.pt"), weights_only=False)["t8_8x8"]
-    out = _unet(unet_sd)(c["sample"].half(), torch.tensor(c["timestep"]), c["low_res"].half(),
-                         encoder_hidden_states=c["ctx"].half(), class_labels=c["class_labels"]).sample
-    assert _rel(out, c["out"]) < 5e-3
-
-
 def test_unet_shared_cfg_prefix_host_logic(emulated, unet_sd):
     m = _unet(unet_sd)
     c = torch.load(os.path.join(G, "unet.pt"), weights_only=False)["t3_16x24"]

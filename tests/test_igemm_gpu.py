@@ -346,32 +346,3 @@ def test_groupnorm_of_a_concat_that_is_never_built():
         _check(got, _gn_ref(cat, gamma, beta, 32, 1e-5, True, B), atol=4e-3)
     # a part without statistics -> None (the caller materialises the concat)
     assert ops.group_norm_cat([x, _rand(B, T, H, W, 256)], gamma, beta, 32, 1e-5, silu=True, n_outer=B) is None
-
-
-@pytest.mark.parametrize("M,K,N,act", [(1000, 512, 512, 0), (148 * 2 * 128 + 40, 512, 1536, 0), (40000, 512, 4096, 2),
-                                       (777, 1024, 1024, 0), (300, 512, 192, 0)])
-def test_layernorm_folded_into_the_consuming_linear(M, K, N, act, monkeypatch):
-    """hs = Linear(...) + residual emits per-row {sum, sumsq} slots (ln_stats); the next Linear runs on the RAW hs against
-    W * gamma and applies rstd (acc - mean colsum) + (b + W beta) in its epilogue == Linear(LayerNorm(hs)) of the reference
-    (attention.py:525-563), without the normalised tensor ever existing"""
-    monkeypatch.setattr(ops, "LN_FUSED", True)  # opt-in path (off by default: slower at config 2, see ops.LN_FUSED)
-    torch.manual_seed(7)
-    a0, w0 = _rand(M, 256), _rand(K, 256, scale=0.08)
-    res = _rand(M, K, scale=1.5) + 0.7          # non-zero row means: the rank-1 correction matters
-    hs = ops.linear(a0, w0, torch.randn(K, device=DEV) * 0.1, residual=res, ln_stats=True)
-    st = hs.uav_ln
-    assert st.C == K and st.partial.shape[0] == M
-    # the emitted statistics are those of the stored rows (fp32 values before the fp16 rounding)
-    s_ref = hs.float().sum(-1)
-    assert (st.partial[..., 0].sum(-1) - s_ref).abs().max().item() < 0.05 * K ** 0.5
-    gamma, beta = torch.randn(K, device=DEV) * 0.2 + 1, torch.randn(K, device=DEV) * 0.1
-    W, b = torch.randn(N, K, device=DEV) * 0.05, torch.randn(N, device=DEV) * 0.1
-    wp = (W * gamma[None, :]).half().contiguous()
-    bp = (b + W @ beta).contiguous()
-    colsum = wp.float().sum(dim=1).contiguous()
-    out = ops.linear(hs, wp, bp, ln=(st, colsum, 1e-5), act=act)
-    y = F.linear(F.layer_norm(hs.float(), (K,), gamma, beta, 1e-5), W, b)
-    if act == 2:
-        h, g = y.chunk(2, dim=-1)
-        y = h * F.gelu(g)
-    _check(out, y, atol=6e-3, rtol=4e-3)

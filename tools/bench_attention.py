@@ -12,16 +12,13 @@ def timeit(fn, iters=3, warmup=1):
     for _ in range(iters): fn()
     e.record(); torch.cuda.synchronize()
     return s.elapsed_time(e) / iters
-tag = "hmma" if os.environ.get("UAV_ATTENTION_HMMA") == "1" else "wgmma"
 for name, B, heads, d, n in [("vae d512 N=46080", 1, 1, 512, 46080), ("vae d512 N=184320", 1, 1, 512, 184320),
                              ("unet self d128 N=2880 x16 frames", 16, 8, 128, 2880)]:
-    if tag == "hmma" and n > 100000:
-        continue
     C = heads * d
     qkv = torch.randn(B, n, 3 * C, device="cuda").half()
     out = torch.empty(B, n, C, device="cuda", dtype=torch.float16)
     ms = timeit(lambda: ops.attention(qkv[..., :C], qkv[..., C:2*C], qkv[..., 2*C:], heads, out=out))
-    print(json.dumps({"impl": tag, "name": name, "ms": ms, "tflops_alg": 4.0 * B * n * n * C / ms / 1e9}))
+    print(json.dumps({"name": name, "ms": ms, "tflops_alg": 4.0 * B * n * n * C / ms / 1e9}))
 
 # temporal attention at the top UNet level (B=2, T=8, 160x288, 8 heads x 64): 8 B/element stream
 import math
@@ -35,7 +32,7 @@ rot = torch.stack([ang.cos(), ang.sin()], dim=-1).contiguous().cuda()
 bias = (torch.randn(heads, Fr, Fr) * 0.3).cuda()
 out = torch.empty(B, Fr, HW, C, device="cuda", dtype=torch.float16)
 ms = timeit(lambda: ops.temporal_attention(q, k, v, heads, rot, bias, out=out), iters=10, warmup=3)
-print(json.dumps({"impl": "shfl" if os.environ.get("UAV_TEMPORAL_SHFL") == "1" else "mma", "name": "temporal attn 2x8x46080 h8 d64",
+print(json.dumps({"name": "temporal attn 2x8x46080 h8 d64",
                   "ms": ms, "GBps": 4 * B * Fr * HW * C * 2 / ms / 1e6}))
 
 # text cross-attention at the top UNet level: 16 frames x 46080 queries, 77 keys, 8 heads x 64 (4 B/element stream of q, o)

@@ -1,5 +1,4 @@
-"""GroupNorm(+SiLU) apply pass alone, CUDA events, buffers rotated so that no launch finds its input in L2.
-`UAV_GN_SILU_PAIR=0 python tools/bench_gn.py` vs `python tools/bench_gn.py` is the A/B of the shared-reciprocal SiLU."""
+"""GroupNorm(+SiLU) apply pass alone, CUDA events, buffers rotated so that no launch finds its input in L2."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -7,7 +6,6 @@ from upscale_a_video_b200 import ops
 
 dev = torch.device("cuda")
 SHAPES = [(16, 160, 288, 512), (16, 320, 576, 256), (16, 320, 576, 512), (16, 80, 144, 512), (16, 40, 72, 1024)]
-print("UAV_GN_SILU_PAIR =", os.environ.get("UAV_GN_SILU_PAIR", "(default: 1)"))
 for shp in SHAPES:
     n, h, w, c = shp
     nbuf = max(2, int(1.5e9 // (n * h * w * c * 2)) + 1)

@@ -1,12 +1,12 @@
 """per-shape timing of one UNet forward at config 2 (B=2 = the two CFG halves of one clip, T=8, 320x576), as the pipeline
-calls it (cfg_shared_input=True), plus A/B totals of the round-2 switches toggled in-process.  usage: profile_unet.py [--ab]"""
+calls it (cfg_shared_input=True)"""
 import json
 import os
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
-from upscale_a_video_b200 import UNetVideoModel, layers, ops
+from upscale_a_video_b200 import UNetVideoModel, ops
 from upscale_a_video_b200.synthetic import seeded_state_dict
 
 dev = torch.device("cuda")
@@ -40,21 +40,3 @@ def run(tag, detail=False):
 
 
 run("default", detail=True)
-if "--ab" in sys.argv:
-    from upscale_a_video_b200 import unet_video
-    layers.GN_STATS_LINEAR = False
-    run("no statistics from Linear / 1x1 producers (UAV_GN_STATS_LINEAR=0)")
-    layers.GN_STATS_LINEAR = True
-    layers.VIRTUAL_CONCAT = False
-    run("concat buffers, main branch in place (UAV_VIRTUAL_CONCAT=0)")
-    layers.GN_STATS_LINEAR = False
-    run("UAV_VIRTUAL_CONCAT=0 + UAV_GN_STATS_LINEAR=0")
-    layers.GN_STATS_LINEAR = True
-    layers.VIRTUAL_CONCAT = True
-    unet_video.FUSED_CONV_OUT = False
-    run("separate conv_norm_out / conv_out kernels (UAV_FUSED_CONV_OUT=0)")
-    unet_video.FUSED_CONV_OUT = True
-    ops.GN_FUSED_STATS = False
-    run("GN statistics by their own pass (UAV_GN_FUSED_STATS=0)")
-    ops.GN_FUSED_STATS = True
-    run("default again")

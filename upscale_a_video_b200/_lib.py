@@ -38,12 +38,6 @@ class Epilogue(C.Structure):
         ("out_scale", C.c_float),
         ("gn_partial", C.c_void_p),
         ("gn_blocks", C.c_int64),
-        ("ln_in", C.c_void_p),
-        ("ln_colsum", C.c_void_p),
-        ("ln_slots", C.c_int),
-        ("ln_eps", C.c_float),
-        ("ln_out", C.c_void_p),
-        ("ln_out_slots", C.c_int),
     ]
 
 
@@ -91,8 +85,7 @@ _PROTOS = {
     "uav_ddim_step_v0": [P, P, P, I64, I32, F32, F32, I32, F32, I32, P],
     "uav_ddim_step_vt": [P, P, P, P, I64, I32, F32, F32, F32, F32, I32, F32, F32, P, I32, P],
     "uav_add_noise": [P, P, P, I64, F32, F32, I32, P],
-    "uav_propagate_step": [P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I64, I32, I32, F32, F32, F32,
-                           I32, I32, P],
+    "uav_propagate_step": [P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I64, I32, I32, F32, F32, F32, I32, P],
     "uav_conv2d_taps": [P, I64, I64, I64, I64, I64, P, I64, I32, I32, I32, I32, P, EP, P],
     "uav_instnorm_relu": [P, I64, I64, I64, F32, I32, P, P, P],
     "uav_add_relu": [P, P, P, I64, P],
@@ -116,7 +109,6 @@ _SPECIAL = {
     "uav_launch_count": (C.c_uint64, []),
     "uav_groupnorm_workspace_bytes": (C.c_size_t, [I64, I32]),
     "uav_gn_partial_blocks": (C.c_int64, [I64, I64, I64]),
-    "uav_ln_partial_slots": (C.c_int, [I64]),
     "uav_plane_stats_workspace_bytes": (C.c_size_t, [I64]),
     "uav_instnorm_workspace_bytes": (C.c_size_t, [I64, I64]),
 }

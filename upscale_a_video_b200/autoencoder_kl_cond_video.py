@@ -14,8 +14,6 @@ from typing import Optional, Tuple
 import torch
 from torch import nn
 
-import os
-
 from . import ops
 from ._config import ConfigMixin
 from . import _lib
@@ -28,8 +26,8 @@ from .layers import (Ctx, DownEncoderBlock3D, Fuse_sft_block, InflatedConv3d, Pa
 # (shortcut / upsampler convs, residual adds) or a GroupNorm — scale invariant once its eps is scaled too — so the decoder
 # keeps the stream at 2^-k of the reference's values (fp16 range x 2^k, power-of-two scale = no rounding change) and every
 # branch output (post-GroupNorm, O(1)) is multiplied by 2^-k in the GEMM epilogue that adds it to the stream.  All fp16
-# stores also saturate instead of producing inf.  UAV_VAE_STREAM_SHIFT=0 restores the unscaled stream.
-VAE_STREAM_SCALE = 2.0 ** -int(os.environ.get("UAV_VAE_STREAM_SHIFT", "7"))
+# stores also saturate instead of producing inf.
+VAE_STREAM_SCALE = 2.0 ** -7
 
 
 @dataclass

@@ -2,12 +2,11 @@
 //
 //  * uav_attention: softmax(Q K^T * scale) V without materialising the score matrix
 //    (the reference materialises it: attention.py:209-238, 2.1 GB per call at 320x576).
-//    FlashAttention-2 style tiling on mma.sync.m16n8k16 (fp16 in, fp32 accumulate, fp32
-//    online softmax): used for the UNet spatial self-attention (N = h*w, d = 128), the text
-//    cross-attention (Nk = 77, d = 64/128, K/V shared by all frames of a batch item) and the
-//    VAE mid-block attention (1 head, d = 512, as four 128-wide V slices).
-//    The d = 128 self-attention and the d = 512 VAE attention run on the wgmma kernel of
-//    attention_tc.cu; this mma.sync kernel serves the other head dims (64) and UAV_ATTENTION_HMMA=1.
+//    Short key sequences (the text cross-attention: Nk = 77, d = 64/128, K/V shared by all
+//    frames of a batch item) run on a resident-KV mma.sync kernel.  Otherwise d = 128 (UNet
+//    spatial self-attention, N = h*w) and d = 512 (VAE mid-block attention, 1 head) run on the
+//    wgmma kernel of attention_tc.cu, and d = 64 on a FlashAttention-2 style mma.sync.m16n8k16
+//    kernel (fp16 in, fp32 accumulate, fp32 online softmax).
 //  * uav_temporal_attention: the seq = T <= 8 per-pixel attention with rotary embedding on
 //    the first 32 dims and the T5-style relative-position bias (attention.py:699-733) as a
 //    register-resident warp kernel: one warp per (pixel, head), lane = (frame, quarter of the
@@ -17,16 +16,16 @@
 #include "uav_common.cuh"
 
 #include <atomic>
-#include <stdlib.h>
 
 namespace uav {
 extern std::atomic<uint64_t> g_launches;
 
 // ---------------------------------------------------------------------------------------
-// flash attention (mma.sync)
+// flash attention (mma.sync), d = 64
 // ---------------------------------------------------------------------------------------
 constexpr int FA_BM = 64;   // query rows per CTA (4 warps x 16)
 constexpr int FA_BN = 64;   // kv rows per iteration
+constexpr int FA_D = 64;    // head dim
 constexpr int FA_THREADS = 128;
 
 struct FaParams {
@@ -78,46 +77,44 @@ __device__ __forceinline__ __half* tile_ptr(__half* base, int row, int chunk) {
   return base + row * DT + ((chunk ^ (row & 7)) << 3);
 }
 
-// DQK: head dim of q/k; DV: width of the V slice processed by this launch
-template <int DQK, int DV>
 __global__ void __launch_bounds__(FA_THREADS)
     flash_attn_kernel(const FaParams p) {
   extern __shared__ __align__(16) uint8_t fa_smem[];
-  __half* sq = reinterpret_cast<__half*>(fa_smem);  // [64][DQK]
-  __half* sk = sq + FA_BM * DQK;                    // [2][64][DQK]
-  __half* sv = sk + 2 * FA_BN * DQK;                // [2][64][DV]
+  __half* sq = reinterpret_cast<__half*>(fa_smem);  // [64][FA_D]
+  __half* sk = sq + FA_BM * FA_D;                   // [2][64][FA_D]
+  __half* sv = sk + 2 * FA_BN * FA_D;               // [2][64][FA_D]
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int bh = blockIdx.y;
   const int b = bh / p.heads, h = bh % p.heads;
   const int q0 = blockIdx.x * FA_BM;
-  const __half* qg = p.q + b * p.bsq + static_cast<int64_t>(h) * DQK;
-  const __half* kg = p.k + (b / p.kv_batch_div) * p.bsk + static_cast<int64_t>(h) * DQK;
-  const __half* vg = p.v + (b / p.kv_batch_div) * p.bsv + static_cast<int64_t>(h) * DV;
-  __half* og = p.o + b * p.bso + static_cast<int64_t>(h) * DV;
+  const __half* qg = p.q + b * p.bsq + static_cast<int64_t>(h) * FA_D;
+  const __half* kg = p.k + (b / p.kv_batch_div) * p.bsk + static_cast<int64_t>(h) * FA_D;
+  const __half* vg = p.v + (b / p.kv_batch_div) * p.bsv + static_cast<int64_t>(h) * FA_D;
+  __half* og = p.o + b * p.bso + static_cast<int64_t>(h) * FA_D;
 
-  constexpr int QC = DQK / 8, VC = DV / 8;  // 16B chunks per row
+  constexpr int QC = FA_D / 8;  // 16B chunks per row
   // ---- async loads: Q tile, then K/V tile 0 ----
   for (int i = tid; i < FA_BM * QC; i += FA_THREADS) {
     const int r = i / QC, c = i % QC;
     const bool ok = q0 + r < p.nq;
-    cp_async16(tile_ptr<DQK>(sq, r, c), qg + static_cast<int64_t>(ok ? q0 + r : 0) * p.ldq + c * 8,
+    cp_async16(tile_ptr<FA_D>(sq, r, c), qg + static_cast<int64_t>(ok ? q0 + r : 0) * p.ldq + c * 8,
                ok);
   }
   auto load_kv = [&](int tile, int buf) {
     const int k0 = tile * FA_BN;
-    __half* skb = sk + buf * FA_BN * DQK;
-    __half* svb = sv + buf * FA_BN * DV;
+    __half* skb = sk + buf * FA_BN * FA_D;
+    __half* svb = sv + buf * FA_BN * FA_D;
     for (int i = tid; i < FA_BN * QC; i += FA_THREADS) {
       const int r = i / QC, c = i % QC;
       const bool ok = k0 + r < p.nk;
-      cp_async16(tile_ptr<DQK>(skb, r, c),
+      cp_async16(tile_ptr<FA_D>(skb, r, c),
                  kg + static_cast<int64_t>(ok ? k0 + r : 0) * p.ldk + c * 8, ok);
     }
-    for (int i = tid; i < FA_BN * VC; i += FA_THREADS) {
-      const int r = i / VC, c = i % VC;
+    for (int i = tid; i < FA_BN * QC; i += FA_THREADS) {
+      const int r = i / QC, c = i % QC;
       const bool ok = k0 + r < p.nk;
-      cp_async16(tile_ptr<DV>(svb, r, c),
+      cp_async16(tile_ptr<FA_D>(svb, r, c),
                  vg + static_cast<int64_t>(ok ? k0 + r : 0) * p.ldv + c * 8, ok);
     }
   };
@@ -125,9 +122,9 @@ __global__ void __launch_bounds__(FA_THREADS)
   cp_async_commit();
 
   const int ntiles = (p.nk + FA_BN - 1) / FA_BN;
-  float o_acc[DV / 8][4];
+  float o_acc[FA_D / 8][4];
 #pragma unroll
-  for (int i = 0; i < DV / 8; ++i) o_acc[i][0] = o_acc[i][1] = o_acc[i][2] = o_acc[i][3] = 0.f;
+  for (int i = 0; i < FA_D / 8; ++i) o_acc[i][0] = o_acc[i][1] = o_acc[i][2] = o_acc[i][3] = 0.f;
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
 
   const int g = lane >> 2, t4 = lane & 3;
@@ -140,23 +137,23 @@ __global__ void __launch_bounds__(FA_THREADS)
     cp_async_commit();
     cp_async_wait<1>();
     __syncthreads();
-    const __half* skb = sk + buf * FA_BN * DQK;
-    const __half* svb = sv + buf * FA_BN * DV;
+    const __half* skb = sk + buf * FA_BN * FA_D;
+    const __half* svb = sv + buf * FA_BN * FA_D;
 
     // ---- S = Q K^T (16 x 64 per warp) ----
     float s[FA_BN / 8][4];
 #pragma unroll
     for (int i = 0; i < FA_BN / 8; ++i) s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f;
 #pragma unroll
-    for (int kk = 0; kk < DQK / 16; ++kk) {
+    for (int kk = 0; kk < FA_D / 16; ++kk) {
       uint32_t a[4];
-      ldmatrix_x4(a, tile_ptr<DQK>(sq, arow, kk * 2 + achk));
+      ldmatrix_x4(a, tile_ptr<FA_D>(sq, arow, kk * 2 + achk));
 #pragma unroll
       for (int nb = 0; nb < FA_BN / 16; ++nb) {
         uint32_t bfr[4];
         const int brow = nb * 16 + (lane & 7) + (lane >> 4) * 8;
         const int bchk = kk * 2 + ((lane >> 3) & 1);
-        ldmatrix_x4(bfr, tile_ptr<DQK>(const_cast<__half*>(skb), brow, bchk));
+        ldmatrix_x4(bfr, tile_ptr<FA_D>(const_cast<__half*>(skb), brow, bchk));
         mma16816(s[nb * 2], a, bfr[0], bfr[1]);
         mma16816(s[nb * 2 + 1], a, bfr[2], bfr[3]);
       }
@@ -201,7 +198,7 @@ __global__ void __launch_bounds__(FA_THREADS)
 #pragma unroll
     for (int r = 0; r < 2; ++r) l_run[r] = l_run[r] * corr[r] + rs[r];
 #pragma unroll
-    for (int i = 0; i < DV / 8; ++i) {
+    for (int i = 0; i < FA_D / 8; ++i) {
       o_acc[i][0] *= corr[0];
       o_acc[i][1] *= corr[0];
       o_acc[i][2] *= corr[1];
@@ -212,11 +209,11 @@ __global__ void __launch_bounds__(FA_THREADS)
     for (int kk = 0; kk < FA_BN / 16; ++kk) {
       const uint32_t a[4] = {pf[kk * 2][0], pf[kk * 2][1], pf[kk * 2 + 1][0], pf[kk * 2 + 1][1]};
 #pragma unroll
-      for (int nb = 0; nb < DV / 16; ++nb) {
+      for (int nb = 0; nb < FA_D / 16; ++nb) {
         uint32_t bfr[4];
         const int vrow = kk * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
         const int vchk = nb * 2 + (lane >> 4);
-        ldmatrix_x4_trans(bfr, tile_ptr<DV>(const_cast<__half*>(svb), vrow, vchk));
+        ldmatrix_x4_trans(bfr, tile_ptr<FA_D>(const_cast<__half*>(svb), vrow, vchk));
         mma16816(o_acc[nb * 2], a, bfr[0], bfr[1]);
         mma16816(o_acc[nb * 2 + 1], a, bfr[2], bfr[3]);
       }
@@ -225,7 +222,7 @@ __global__ void __launch_bounds__(FA_THREADS)
   }
   cp_async_wait<0>();
 
-  // ---- finalize: O / l -> smem (reuse Q tile region, needs DV <= DQK) -> coalesced stores ----
+  // ---- finalize: O / l -> smem (reuse Q tile region) -> coalesced stores ----
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     float l = l_run[r];
@@ -233,21 +230,21 @@ __global__ void __launch_bounds__(FA_THREADS)
     l += __shfl_xor_sync(0xffffffff, l, 2);
     l_run[r] = (l > 0.f) ? 1.f / l : 0.f;
   }
-  __half* so = sq;  // [64][DV] swizzled like a DV tile
+  __half* so = sq;  // [64][FA_D]
 #pragma unroll
-  for (int nb = 0; nb < DV / 8; ++nb) {
+  for (int nb = 0; nb < FA_D / 8; ++nb) {
     const int r0 = warp * 16 + g, r1 = r0 + 8;
     __half2 v0 = __floats2half2_rn(o_acc[nb][0] * l_run[0], o_acc[nb][1] * l_run[0]);
     __half2 v1 = __floats2half2_rn(o_acc[nb][2] * l_run[1], o_acc[nb][3] * l_run[1]);
-    *reinterpret_cast<__half2*>(tile_ptr<DV>(so, r0, nb) + t4 * 2) = v0;
-    *reinterpret_cast<__half2*>(tile_ptr<DV>(so, r1, nb) + t4 * 2) = v1;
+    *reinterpret_cast<__half2*>(tile_ptr<FA_D>(so, r0, nb) + t4 * 2) = v0;
+    *reinterpret_cast<__half2*>(tile_ptr<FA_D>(so, r1, nb) + t4 * 2) = v1;
   }
   __syncthreads();
-  for (int i = tid; i < FA_BM * VC; i += FA_THREADS) {
-    const int r = i / VC, c = i % VC;
+  for (int i = tid; i < FA_BM * QC; i += FA_THREADS) {
+    const int r = i / QC, c = i % QC;
     if (q0 + r < p.nq)
       stg16(og + static_cast<int64_t>(q0 + r) * p.ldo + c * 8,
-            *reinterpret_cast<const uint4*>(tile_ptr<DV>(so, r, c)));
+            *reinterpret_cast<const uint4*>(tile_ptr<FA_D>(so, r, c)));
   }
 }
 
@@ -723,18 +720,16 @@ uav_status_t attention_tc(const void* q, const void* k, const void* v, void* out
                           int64_t ldv, int64_t ldo, int64_t kv_batch_div, float scale,
                           cudaStream_t stream);  // attention_tc.cu (wgmma)
 
-template <int DQK, int DV>
 static uav_status_t launch_fa(const FaParams& p, int batch, cudaStream_t stream) {
-  constexpr int smem = (FA_BM * DQK + 2 * FA_BN * DQK + 2 * FA_BN * DV) * 2;
+  constexpr int smem = (FA_BM + 4 * FA_BN) * FA_D * 2;
   static uint64_t configured = 0;  // per-device bit: cudaFuncSetAttribute applies to the current device only
   const uint64_t dev_bit = 1ull << (current_device() & 63);
   if (!(configured & dev_bit)) {
-    UAV_CHECK_CUDA(cudaFuncSetAttribute(flash_attn_kernel<DQK, DV>,
-                                        cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    UAV_CHECK_CUDA(cudaFuncSetAttribute(flash_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     configured |= dev_bit;
   }
   dim3 grid((p.nq + FA_BM - 1) / FA_BM, batch * p.heads);
-  flash_attn_kernel<DQK, DV><<<grid, FA_THREADS, smem, stream>>>(p);
+  flash_attn_kernel<<<grid, FA_THREADS, smem, stream>>>(p);
   UAV_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(1, std::memory_order_relaxed);
   return UAV_OK;
@@ -758,10 +753,7 @@ uav_status_t uav_attention(const void* q, const void* k, const void* v, void* ou
               "uav_attention: token strides must be multiples of 8");
   UAV_REQUIRE(batch * heads <= 65535, "uav_attention: batch*heads too large");
   UAV_REQUIRE(batch % kv_batch_div == 0, "uav_attention: batch must be a multiple of kv_batch_div");
-  // d = 128 (UNet self / cross attention at h/8) and d = 512 (VAE AttentionBlock) run on the wgmma
-  // kernel; UAV_ATTENTION_HMMA=1 selects the mma.sync kernel instead (kept for A/B measurements)
-  static const bool no_cross = getenv("UAV_ATTENTION_NOCROSS") != nullptr && getenv("UAV_ATTENTION_NOCROSS")[0] == '1';
-  if (!no_cross && nk <= 128 && nq >= 4 * nk && (head_dim == 64 || head_dim == 128)) {
+  if (nk <= 128 && nq >= 4 * nk && (head_dim == 64 || head_dim == 128)) {
     // short key/value sequence (the 77 prompt tokens): resident-KV streaming kernel
     FaParams pc;
     pc.q = (const __half*)q; pc.k = (const __half*)k; pc.v = (const __half*)v; pc.o = (__half*)out;
@@ -772,32 +764,21 @@ uav_status_t uav_attention(const void* q, const void* k, const void* v, void* ou
     if (head_dim == 64) return nk <= 80 ? launch_cross<64, 5>(pc, (int)batch, stream) : launch_cross<64, 8>(pc, (int)batch, stream);
     return nk <= 80 ? launch_cross<128, 5>(pc, (int)batch, stream) : launch_cross<128, 8>(pc, (int)batch, stream);
   }
-  static const bool force_hmma = getenv("UAV_ATTENTION_HMMA") != nullptr && getenv("UAV_ATTENTION_HMMA")[0] == '1';
-  if (!force_hmma && (head_dim == 128 || head_dim == 512))
+  // d = 128 (UNet self-attention at h/8) and d = 512 (VAE AttentionBlock) run on the wgmma kernel
+  if (head_dim == 128 || head_dim == 512)
     return attention_tc(q, k, v, out, batch, heads, head_dim, nq, nk, ldq, ldk, ldv, ldo, kv_batch_div, scale,
                         stream);
-  FaParams p;
-  p.q = (const __half*)q;
-  p.k = (const __half*)k;
-  p.v = (const __half*)v;
-  p.o = (__half*)out;
-  p.ldq = ldq; p.ldk = ldk; p.ldv = ldv; p.ldo = ldo;
-  p.bsq = nq * ldq; p.bsk = nk * ldk; p.bsv = nk * ldv; p.bso = nq * ldo;
-  p.nq = (int)nq; p.nk = (int)nk; p.heads = heads; p.kv_batch_div = (int)kv_batch_div;
-  p.scale_log2 = scale * 1.4426950408889634f;
-  if (head_dim == 64) return launch_fa<64, 64>(p, (int)batch, stream);
-  if (head_dim == 128) return launch_fa<128, 128>(p, (int)batch, stream);
-  if (head_dim == 512) {
-    // single wide head (VAE AttentionBlock): four passes over 128-wide V / output slices
-    UAV_REQUIRE(heads == 1, "uav_attention: head_dim 512 supports a single head");
-    for (int s = 0; s < 4; ++s) {
-      FaParams ps = p;
-      ps.v = p.v + s * 128;
-      ps.o = p.o + s * 128;
-      uav_status_t st = launch_fa<512, 128>(ps, (int)batch, stream);
-      if (st != UAV_OK) return st;
-    }
-    return UAV_OK;
+  if (head_dim == 64) {
+    FaParams p;
+    p.q = (const __half*)q;
+    p.k = (const __half*)k;
+    p.v = (const __half*)v;
+    p.o = (__half*)out;
+    p.ldq = ldq; p.ldk = ldk; p.ldv = ldv; p.ldo = ldo;
+    p.bsq = nq * ldq; p.bsk = nk * ldk; p.bsv = nk * ldv; p.bso = nq * ldo;
+    p.nq = (int)nq; p.nk = (int)nk; p.heads = heads; p.kv_batch_div = (int)kv_batch_div;
+    p.scale_log2 = scale * 1.4426950408889634f;
+    return launch_fa(p, (int)batch, stream);
   }
   set_last_error("uav_attention: head_dim %d unsupported (64, 128, 512)", head_dim);
   return UAV_ERR_UNSUPPORTED;
@@ -822,8 +803,7 @@ uav_status_t uav_temporal_attention(const void* q, const void* k, const void* v,
   p.scale = scale; p.rot = rot_cos_sin; p.bias = rel_bias;
   const int64_t warps = B * HW * heads;
   const unsigned grid = (unsigned)((warps + 7) / 8);
-  static const bool force_shfl = getenv("UAV_TEMPORAL_SHFL") && getenv("UAV_TEMPORAL_SHFL")[0] == '1';
-  if (heads % 2 == 0 && !force_shfl && (head_dim == 64 || head_dim == 128)) {
+  if (heads % 2 == 0 && (head_dim == 64 || head_dim == 128)) {
     // mma.sync formulation: one warp per pair of heads
     const unsigned grid2 = (unsigned)((warps / 2 + 3) / 4);
     if (head_dim == 64) temporal_attn_mma_kernel<64><<<grid2, 128, 0, stream>>>(p);

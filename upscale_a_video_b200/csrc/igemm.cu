@@ -113,14 +113,6 @@ struct alignas(64) IgemmParams {
   float out_scale;     // applied before the residual add (1 = off)
   float* gn_partial;   // [n_out / 8][gn_blocks][2] GroupNorm statistics of the output, or nullptr
   int64_t gn_blocks;
-  // LayerNorm folded into the GEMM (see uav_epilogue_t): per-row {sum, sumsq} slots of the INPUT rows written by its
-  // producer, the column sums of the gamma-scaled weight, and (as a producer) the slots of the OUTPUT rows
-  const float2* ln_in;
-  const float* ln_colsum;
-  int32_t ln_slots;
-  float ln_inv_c, ln_eps;
-  float2* ln_out;
-  int32_t ln_out_slots;
 };
 
 template <int BLOCK_N, bool GEGLU>
@@ -156,10 +148,6 @@ __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o >= 1; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
-}
-__device__ __forceinline__ float quad_sum(float v) {
-  v += __shfl_xor_sync(0xffffffffu, v, 1);
-  return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
 // TMA_EPI: smem-staged TMA-store epilogue (aligned fp16 output, >= 64-column tiles) vs direct per-element stores.
@@ -335,7 +323,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
     int64_t out_row[2];
     const __half* rv[2];
     const __half* res[2];
-    float ln_a[2] = {1.f, 1.f}, ln_b[2] = {0.f, 0.f};
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const uint32_t o1 = t1 + l1[h], o2 = t2 + l2[h], o3 = t3 + l3[h], o4 = t4 + l4[h];
@@ -344,25 +331,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
       rv[h] = (AUX && p.rowvec != nullptr && row_ok[h]) ? p.rowvec + (out_row[h] / p.rows_per_vec) * p.ld_rowvec
                                                          : nullptr;
       res[h] = (AUX && !TMA_EPI && p.residual != nullptr && row_ok[h]) ? p.residual + out_row[h] * p.ld_res : nullptr;
-      if constexpr (AUX) {
-        // LayerNorm of the input rows folded into this GEMM: acc was computed on the RAW rows x against W' = W * gamma, so
-        // LN(x) W^T + b = rstd * (acc - mean * colsum(W')) + b'  with the row statistics emitted by x's producer
-        if (p.ln_in != nullptr) {
-          float s_ = 0.f, q_ = 0.f;
-          if (row_ok[h]) {
-            const float2* lp = p.ln_in + out_row[h] * p.ln_slots;
-            for (int i = 0; i < p.ln_slots; ++i) {
-              const float2 t = __ldg(lp + i);
-              s_ += t.x;
-              q_ += t.y;
-            }
-          }
-          const float mean = s_ * p.ln_inv_c;
-          const float var = fmaxf(fmaf(-mean, mean, q_ * p.ln_inv_c), 0.f);
-          ln_a[h] = rsqrtf(var + p.ln_eps);
-          ln_b[h] = -mean * ln_a[h];
-        }
-      }
     }
     if constexpr (TMA_EPI) {
       epi_bar_sync();  // thread 0 saw the previous store release the staging tile
@@ -373,28 +341,18 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
         }
       }
     }
-    float ln_s[2][2] = {{0.f, 0.f}, {0.f, 0.f}}, ln_q[2][2] = {{0.f, 0.f}, {0.f, 0.f}};  // [row][column half]
 #pragma unroll
     for (int jb = 0; jb < OUT_TILE_N / 8; ++jb) {
       const int col = jb * 8 + 2 * lr;  // column inside the output tile (this thread: col, col + 1)
       const int n = n_base + col;
       const bool ok0 = n < p.n_out, ok1 = n + 1 < p.n_out;
-      float b0 = 0.f, b1 = 0.f, g0 = 0.f, g1 = 0.f, cs0 = 0.f, cs1 = 0.f, cg0 = 0.f, cg1 = 0.f;
+      float b0 = 0.f, b1 = 0.f, g0 = 0.f, g1 = 0.f;
       if (p.bias != nullptr) {
         if (ok0) b0 = __ldg(p.bias + n);
         if (ok1) b1 = __ldg(p.bias + n + 1);
         if (GEGLU) {
           if (ok0) g0 = __ldg(p.bias + p.N / 2 + n);
           if (ok1) g1 = __ldg(p.bias + p.N / 2 + n + 1);
-        }
-      }
-      const bool ln_fold = AUX && p.ln_in != nullptr;
-      if (ln_fold) {
-        if (ok0) cs0 = __ldg(p.ln_colsum + n);
-        if (ok1) cs1 = __ldg(p.ln_colsum + n + 1);
-        if (GEGLU) {
-          if (ok0) cg0 = __ldg(p.ln_colsum + p.N / 2 + n);
-          if (ok1) cg1 = __ldg(p.ln_colsum + p.N / 2 + n + 1);
         }
       }
       float gs = 0.f, gq = 0.f;  // GroupNorm statistics of this 8-column group over the thread's rows
@@ -405,21 +363,11 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
         if constexpr (GEGLU) {
           constexpr int GJ = OUT_TILE_N / 8;  // gate columns start at accumulator column OUT_TILE_N
           const float q0 = acc[4 * (jb + GJ) + 2 * h], q1 = acc[4 * (jb + GJ) + 2 * h + 1];
-          if (ln_fold) {
-            x0 = fmaf(a0, ln_a[h], fmaf(cs0, ln_b[h], b0)) * gelu_erf_f(fmaf(q0, ln_a[h], fmaf(cg0, ln_b[h], g0)));
-            x1 = fmaf(a1, ln_a[h], fmaf(cs1, ln_b[h], b1)) * gelu_erf_f(fmaf(q1, ln_a[h], fmaf(cg1, ln_b[h], g1)));
-          } else {
-            x0 = (a0 + b0) * gelu_erf_f(q0 + g0);
-            x1 = (a1 + b1) * gelu_erf_f(q1 + g1);
-          }
+          x0 = (a0 + b0) * gelu_erf_f(q0 + g0);
+          x1 = (a1 + b1) * gelu_erf_f(q1 + g1);
         } else {
-          if (ln_fold) {
-            x0 = fmaf(a0, ln_a[h], fmaf(cs0, ln_b[h], b0));
-            x1 = fmaf(a1, ln_a[h], fmaf(cs1, ln_b[h], b1));
-          } else {
-            x0 = a0 + b0;
-            x1 = a1 + b1;
-          }
+          x0 = a0 + b0;
+          x1 = a1 + b1;
         }
         // staging address of (row, col): 16-byte chunk (col & 63) / 8 of the row, CU_TENSOR_MAP_SWIZZLE_128B
         const uint32_t row = lrow[h];
@@ -443,11 +391,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
           } else if (p.out_scale != 1.0f) {
             x0 *= p.out_scale;
             x1 *= p.out_scale;
-          }
-          if (TMA_EPI && p.ln_out != nullptr && ok0) {  // n_out % 8 == 0 on this path: ok0 == ok1
-            const int hf = col >= OUT_TILE_N / 2;
-            ln_s[h][hf] += x0 + x1;
-            ln_q[h][hf] = fmaf(x0, x0, fmaf(x1, x1, ln_q[h][hf]));
           }
           if (row_ok[h] && ok0) {
             gs += x0 + x1;
@@ -479,17 +422,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
             p.gn_partial[(static_cast<int64_t>(oct) * p.gn_blocks + blk) * 2 + 1] = gq;
           }
         }
-      }
-    }
-    if constexpr (AUX && TMA_EPI) {
-      if (p.ln_out != nullptr) {
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-#pragma unroll
-          for (int hf = 0; hf < 2; ++hf) {
-            const float s_ = quad_sum(ln_s[h][hf]), q_ = quad_sum(ln_q[h][hf]);
-            if (lr == 0 && row_ok[h]) p.ln_out[out_row[h] * p.ln_out_slots + n_tile * 2 + hf] = make_float2(s_, q_);
-          }
       }
     }
     if constexpr (TMA_EPI) {
@@ -557,7 +489,7 @@ static uav_status_t launch_instance2(IgemmParams& p, cudaStream_t stream) {
 template <int BLOCK_N, bool GEGLU>
 static uav_status_t launch_instance(IgemmParams& p, cudaStream_t stream) {
   const bool aux = p.rowvec != nullptr || p.residual != nullptr || (p.act != UAV_ACT_NONE && p.act != UAV_ACT_GEGLU) ||
-                   p.out_scale != 1.0f || p.gn_partial != nullptr || p.ln_in != nullptr || p.ln_out != nullptr;
+                   p.out_scale != 1.0f || p.gn_partial != nullptr;
   if constexpr (IgemmCfg<BLOCK_N, GEGLU>::OUT_TILE_N >= 64) {
     if (p.tma_store) {
       return aux ? launch_instance2<BLOCK_N, GEGLU, true, true>(p, stream)
@@ -667,13 +599,6 @@ static uav_status_t launch_igemm(const IgemmDesc& d, cudaStream_t stream) {
   p.out_scale = e->out_scale == 0.0f ? 1.0f : e->out_scale;
   p.gn_partial = reinterpret_cast<float*>(e->gn_partial);
   p.gn_blocks = e->gn_blocks;
-  p.ln_in = reinterpret_cast<const float2*>(e->ln_in);
-  p.ln_colsum = e->ln_colsum;
-  p.ln_slots = e->ln_slots;
-  p.ln_inv_c = 1.0f / static_cast<float>(d.k_per_tap);
-  p.ln_eps = e->ln_eps;
-  p.ln_out = reinterpret_cast<float2*>(e->ln_out);
-  p.ln_out_slots = 0;
   UAV_REQUIRE(!(geglu && p.out_scale != 1.0f), "igemm: out_scale is not supported with GEGLU");
   UAV_REQUIRE(p.ld_out >= p.n_out, "igemm: ld_out (%lld) < output columns (%d)",
               (long long)p.ld_out, p.n_out);
@@ -684,17 +609,6 @@ static uav_status_t launch_igemm(const IgemmDesc& d, cudaStream_t stream) {
   // TMA-store epilogue (smem-staged, fully coalesced, clips partial tiles) whenever the output
   // is an aligned fp16 tensor with at least 64-column tiles; otherwise per-row direct stores.
   p.tma_store = can_tma ? 1 : 0;
-  if (p.ln_in != nullptr || p.ln_out != nullptr) {
-    UAV_REQUIRE(can_tma && d.num_taps == 1 && d.out_strides[1] == 0,
-                "igemm: LayerNorm folding needs a Linear (single tap) with the dense fp16 TMA-store epilogue");
-    UAV_REQUIRE(p.ln_in == nullptr || (p.ln_colsum != nullptr && p.ln_slots >= 1 && p.ln_slots <= 16 &&
-                                       (reinterpret_cast<uintptr_t>(p.ln_colsum) & 15) == 0),
-                "igemm: ln_in needs ln_colsum (16-byte aligned) and 1..16 slots");
-    UAV_REQUIRE(p.ln_out == nullptr || !geglu, "igemm: ln_out is not supported with GEGLU");
-    p.ln_out_slots = (int32_t)p.n_tiles * 2;
-    UAV_REQUIRE(p.ln_out == nullptr || e->ln_out_slots == p.ln_out_slots,
-                "igemm: ln_out_slots is %d, this launch writes %d slots per row", e->ln_out_slots, p.ln_out_slots);
-  }
   if (p.gn_partial != nullptr) {
     UAV_REQUIRE(can_tma && !geglu && d.out_strides[1] == 0,
                 "igemm: GroupNorm statistics need the dense fp16 TMA-store epilogue (n_out >= 33, 16-byte aligned) without GEGLU");
@@ -760,13 +674,6 @@ static void pick_tile_2d(int64_t W, int64_t H, uint32_t* tw, uint32_t* th) {
 using namespace uav;
 
 extern "C" {
-
-int uav_ln_partial_slots(int64_t n_out) {
-  // two column halves per N-tile of the TMA-store epilogue (tile width 128 for N > 64, else 64)
-  if (n_out <= 0) return 0;
-  const int tile = n_out > 64 ? 128 : 64;
-  return (int)((n_out + tile - 1) / tile) * 2;
-}
 
 int64_t uav_gn_partial_blocks(int64_t w, int64_t h, int64_t images) {
   if (w <= 0 || h <= 0 || images <= 0) return 0;

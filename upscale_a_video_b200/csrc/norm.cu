@@ -10,7 +10,6 @@
 
 #include <atomic>
 #include <limits.h>
-#include <stdlib.h>
 #include <string.h>
 
 namespace uav {
@@ -276,12 +275,7 @@ __global__ void __launch_bounds__(GN_THREADS)
       const float2 f = __half22float2(h[j]);
       float a = f.x * sc[2 * j] + sh[2 * j];
       float b = f.y * sc[2 * j + 1] + sh[2 * j + 1];
-      if (silu == 2) {
-        silu2_f(a, b);
-      } else if (silu) {
-        a = silu_f(a);
-        b = silu_f(b);
-      }
+      if (silu) silu2_f(a, b);  // two values per reciprocal (uav_common.cuh)
       ow[j] = pack_half2_sat(a, b);
     }
     stg16(yn + p * ld_out, o);
@@ -476,16 +470,6 @@ __global__ void __launch_bounds__(256)
 
 using namespace uav;
 
-// SiLU flavour of the vectorised apply pass: 2 = two values per reciprocal (uav_common.cuh: silu2_f), 1 = one each.
-// UAV_GN_SILU_PAIR=0 selects the latter (A/B measurements only).
-static int apply_silu_mode(int silu) {
-  static const int pair = [] {
-    const char* e = getenv("UAV_GN_SILU_PAIR");
-    return (e && e[0] == '0') ? 0 : 1;
-  }();
-  return silu ? (pair ? 2 : 1) : 0;
-}
-
 extern "C" {
 
 static constexpr int GN_MAX_BLOCKS_PER_N = 2048;  // upper bound of gridDim.x of the stats kernels
@@ -554,7 +538,7 @@ uav_status_t uav_groupnorm_silu(const void* x, int64_t n_outer, int64_t pixels, 
       int64_t gxa = want < maxb ? want : maxb;
       if (gxa < 1) gxa = 1;
       gn_apply_vec_kernel<<<dim3((unsigned)gxa, (unsigned)n_outer), GN_THREADS, 0, stream>>>(
-          reinterpret_cast<const __half*>(x), pixels, (int)C, ld_in, groups, sums, 1, gamma, beta, eps, apply_silu_mode(silu),
+          reinterpret_cast<const __half*>(x), pixels, (int)C, ld_in, groups, sums, 1, gamma, beta, eps, silu,
           reinterpret_cast<__half*>(y), ld_out, (int)C, 0, pixels * ld_in);
     } else {
       const int64_t work = pixels * C;
@@ -698,7 +682,7 @@ uav_status_t uav_groupnorm_silu_from_partials(const void* x, int64_t n_outer, in
     int64_t gxa = want < maxb ? want : maxb;
     if (gxa < 1) gxa = 1;
     gn_apply_vec_kernel<<<dim3((unsigned)gxa, (unsigned)n_outer), GN_THREADS, 0, stream>>>(
-        xs, pixels, (int)Cs, lds, groups, sums, (int)S, gamma, beta, eps, apply_silu_mode(silu), reinterpret_cast<__half*>(y), ld_out, (int)C,
+        xs, pixels, (int)Cs, lds, groups, sums, (int)S, gamma, beta, eps, silu, reinterpret_cast<__half*>(y), ld_out, (int)C,
         chan, slab_stride);
     UAV_CHECK_CUDA(cudaGetLastError());
     chan += (int)Cs;

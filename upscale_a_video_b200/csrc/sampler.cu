@@ -151,33 +151,29 @@ __global__ void add_noise_kernel(const void* x_, const void* nz_, void* out_, in
 //   fuse:  warped = warped * fuse_scale + cur * (1 - fuse_scale)
 //   out = mask * warped + (1 - mask) * cur
 // feat_* are (C, H, W) planes of one frame (frame stride given), flows are (2, H, W).
-// `half_gs` selects how torch's CUDA grid_sampler treats half inputs: 0 = opmath (fp32
-// coordinates / weights, one final rounding), 1 = every intermediate rounded to half.
+// Grid sampling follows torch's CUDA grid_sampler for half inputs in opmath: fp32 coordinates
+// and weights, one final rounding.
 // ---------------------------------------------------------------------------------------
 template <bool HALF>
 struct GridSample {
   using N = Num<HALF>;
   // source index from a normalised coordinate, align_corners=True
-  static __device__ __forceinline__ float unnorm(float coord, int size, int half_gs) {
-    const float v = __fmul_rn(__fadd_rn(coord, 1.f) * 0.5f, static_cast<float>(size - 1));
-    return half_gs ? N::rh(v) : v;
+  static __device__ __forceinline__ float unnorm(float coord, int size) {
+    return __fmul_rn(__fadd_rn(coord, 1.f) * 0.5f, static_cast<float>(size - 1));
   }
   static __device__ __forceinline__ float bilinear(const typename N::T* plane, int H, int W,
-                                                   float ix, float iy, int half_gs) {
+                                                   float ix, float iy) {
     const int ix_nw = static_cast<int>(floorf(ix)), iy_nw = static_cast<int>(floorf(iy));
     const int ix_ne = ix_nw + 1, iy_ne = iy_nw, ix_sw = ix_nw, iy_sw = iy_nw + 1;
     const int ix_se = ix_nw + 1, iy_se = iy_nw + 1;
-    auto r = [&](float v) { return half_gs ? N::rh(v) : v; };
-    const float nw = r(__fmul_rn(r(ix_se - ix), r(iy_se - iy)));
-    const float ne = r(__fmul_rn(r(ix - ix_sw), r(iy_sw - iy)));
-    const float sw = r(__fmul_rn(r(ix_ne - ix), r(iy - iy_ne)));
-    const float se = r(__fmul_rn(r(ix - ix_nw), r(iy - iy_nw)));
+    const float nw = __fmul_rn(ix_se - ix, iy_se - iy);
+    const float ne = __fmul_rn(ix - ix_sw, iy_sw - iy);
+    const float sw = __fmul_rn(ix_ne - ix, iy - iy_ne);
+    const float se = __fmul_rn(ix - ix_nw, iy - iy_nw);
     float acc = 0.f;
     auto in = [&](int y, int x) { return y >= 0 && y < H && x >= 0 && x < W; };
-    // `out_acc += inp * w` in ATen's grid_sampler kernel: an FMA per corner in opmath mode
-    auto accum = [&](float v, float w) {
-      acc = half_gs ? N::rh(__fadd_rn(acc, N::rh(__fmul_rn(v, w)))) : __fmaf_rn(v, w, acc);
-    };
+    // `out_acc += inp * w` in ATen's grid_sampler kernel: an FMA per corner
+    auto accum = [&](float v, float w) { acc = __fmaf_rn(v, w, acc); };
     if (in(iy_nw, ix_nw)) accum(N::ld(plane, (int64_t)iy_nw * W + ix_nw), nw);
     if (in(iy_ne, ix_ne)) accum(N::ld(plane, (int64_t)iy_ne * W + ix_ne), ne);
     if (in(iy_sw, ix_sw)) accum(N::ld(plane, (int64_t)iy_sw * W + ix_sw), sw);
@@ -198,7 +194,7 @@ __global__ void propagate_step_kernel(const void* feat_prop_, const void* feat_c
                                       int C, int H, int W, int64_t cs_prop, int64_t cs_cur,
                                       int64_t cs_out, int64_t cs_fp, int64_t cs_fc, int nearest,
                                       int fuse, float fuse_scale, float alpha1, float alpha2,
-                                      float inv_wm1, float inv_hm1, int half_gs) {
+                                      float inv_wm1, float inv_hm1) {
   using N = Num<HALF>;
   using T = typename N::T;
   using GS = GridSample<HALF>;
@@ -215,10 +211,10 @@ __global__ void propagate_step_kernel(const void* feat_prop_, const void* feat_c
     const float gx = N::add(static_cast<float>(x), fpx), gy = N::add(static_cast<float>(y), fpy);
     const float vx = N::sub(N::mul(N::mul(2.0f, gx), inv_wm1), 1.0f);
     const float vy = N::sub(N::mul(N::mul(2.0f, gy), inv_hm1), 1.0f);
-    const float ix = GS::unnorm(vx, W, half_gs), iy = GS::unnorm(vy, H, half_gs);
+    const float ix = GS::unnorm(vx, W), iy = GS::unnorm(vy, H);
     // fbConsistencyCheck
-    const float bwx = GS::bilinear(flow_check, H, W, ix, iy, half_gs);
-    const float bwy = GS::bilinear(flow_check + cs_fc, H, W, ix, iy, half_gs);
+    const float bwx = GS::bilinear(flow_check, H, W, ix, iy);
+    const float bwy = GS::bilinear(flow_check + cs_fc, H, W, ix, iy);
     const float dx = N::add(fpx, bwx), dy = N::add(fpy, bwy);
     const float lsq_f = N::add(N::mul(fpx, fpx), N::mul(fpy, fpy));
     const float lsq_b = N::add(N::mul(bwx, bwx), N::mul(bwy, bwy));
@@ -228,7 +224,7 @@ __global__ void propagate_step_kernel(const void* feat_prop_, const void* feat_c
     const float mask = (lsq_d < thr) ? 1.f : 0.f;
     for (int c = 0; c < C; ++c) {
       const T* plane = feat_prop + c * cs_prop;
-      float w = nearest ? GS::nearest(plane, H, W, ix, iy) : GS::bilinear(plane, H, W, ix, iy, half_gs);
+      float w = nearest ? GS::nearest(plane, H, W, ix, iy) : GS::bilinear(plane, H, W, ix, iy);
       const float cur = N::ld(feat_cur, c * cs_cur + i);
       if (fuse) w = N::add(N::mul(w, fuse_scale), N::mul(cur, 1.f - fuse_scale));
       const float r = N::add(N::mul(mask, w), N::mul(N::sub(1.f, mask), cur));
@@ -321,8 +317,7 @@ uav_status_t uav_propagate_step(const void* feat_prop, const void* feat_cur, con
                                 const void* flow_check, void* out, int64_t C, int64_t H, int64_t W,
                                 int64_t cs_prop, int64_t cs_cur, int64_t cs_out, int64_t cs_flow_prop,
                                 int64_t cs_flow_check, int nearest, int fuse, float fuse_scale,
-                                float alpha1, float alpha2, int half_grid_sample, int dtype,
-                                uav_stream_t stream) {
+                                float alpha1, float alpha2, int dtype, uav_stream_t stream) {
   UAV_REQUIRE(feat_prop && feat_cur && flow_prop && flow_check && out && C > 0 && H > 0 && W > 0,
               "uav_propagate_step: bad argument");
   const float inv_wm1 = 1.0f / static_cast<float>(W > 1 ? W - 1 : 1);
@@ -330,7 +325,7 @@ uav_status_t uav_propagate_step(const void* feat_prop, const void* feat_cur, con
   UAV_DISPATCH_DTYPE(dtype, propagate_step_kernel, sgrid(H * W), stream, feat_prop, feat_cur,
                      flow_prop, flow_check, out, (int)C, (int)H, (int)W, cs_prop, cs_cur, cs_out,
                      cs_flow_prop, cs_flow_check, nearest, fuse, fuse_scale, alpha1, alpha2, inv_wm1,
-                     inv_hm1, half_grid_sample);
+                     inv_hm1);
   return UAV_OK;
 }
 

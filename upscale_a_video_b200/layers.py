@@ -17,13 +17,7 @@ from typing import Dict, Optional
 import torch
 from torch import nn
 
-import os
-
 from . import ops
-
-# nearest-x2 upsample fused into the following 3x3 conv (phase-collapsed filters); UAV_FUSE_UPSAMPLE=0 keeps the
-# reference's two-step arithmetic (separate upsample, 9-tap conv)
-FUSE_UPSAMPLE_CONV = os.environ.get("UAV_FUSE_UPSAMPLE", "1") != "0"
 
 
 # ------------------------------------------------------------------------------------------------
@@ -85,19 +79,6 @@ class Packed:
                 b = torch.cat([(m.bias.detach().float() if m.bias is not None else
                                 torch.zeros(m.weight.shape[0], device=w.device)) for m in mods]).contiguous()
             self.cache[key] = (w, b)
-        return self.cache[key]
-
-    def ln_linear(self, key: str, norm: nn.Module, mods):
-        """LayerNorm `norm` folded into the Linear layers `mods` that consume it (row-concatenated like fused_linear):
-        -> (W' = W * gamma fp16 [sum N][K], b' = b + W beta fp32, colsum fp32 [sum N] = sum_k of the fp16 W').
-        LN(x) W^T + b = rstd (x W'^T - mean colsum) + b': the GEMM epilogue applies the right-hand side (ops.linear `ln=`)."""
-        if key not in self.cache:
-            g, bta = norm.weight.detach().float(), norm.bias.detach().float()
-            w = torch.cat([m.weight.detach().float() for m in mods], dim=0)
-            b = torch.cat([(m.bias.detach().float() if m.bias is not None else
-                            torch.zeros(m.weight.shape[0], device=w.device)) for m in mods])
-            wp = (w * g[None, :]).to(torch.float16).contiguous()
-            self.cache[key] = (wp, (b + w @ bta).contiguous(), wp.float().sum(dim=1).contiguous())
         return self.cache[key]
 
     def affine(self, m: nn.Module):
@@ -199,11 +180,6 @@ class InflatedConv3d(nn.Conv2d):
         return ops.conv2d(x, w, b, **kw, **epi)
 
 
-# the producers of GroupNorm inputs emit the statistics from their epilogues (ops.GnStats); Linear / 1x1 producers are
-# short-K GEMMs whose epilogue is the critical path, so they can be excluded separately (UAV_GN_STATS_LINEAR=0)
-GN_STATS_LINEAR = os.environ.get("UAV_GN_STATS_LINEAR", "1") != "0"
-
-
 def _gn(c: Ctx, norm: nn.GroupNorm, x, silu: bool, n_outer: int, stream_scale: float = 1.0):
     """`stream_scale`: x holds stream_scale x the reference's values; GroupNorm(s x) with eps s^2 == GroupNorm(x) with eps"""
     g, b = c.pk.affine(norm)
@@ -236,23 +212,15 @@ def _carry_gn(dst, src):
 # skip-connection concat without the copy of the main branch (unet_blocks.py:573,645 `torch.cat([hidden_states,
 # res_hidden_states], dim=1)`): the concat buffer is allocated BEFORE the layer that produces hidden_states runs, the skip
 # is copied into its tail (a skip computed once for both classifier-free-guidance halves is broadcast there) and the
-# producer's epilogue stores straight into the head slice (`out=`).  UAV_INPLACE_CONCAT=0: two copies, as in round 1.
-INPLACE_CONCAT = os.environ.get("UAV_INPLACE_CONCAT", "1") != "0"
-
-
+# producer's epilogue stores straight into the head slice (`out=`).
 # ... and where both halves carry the GroupNorm statistics of their producers, the concat is never built at all
 # (ResnetBlock3D.forward_cat): norm1 normalises the two tensors straight into ONE dense tensor (ops.group_norm_cat) and the
-# 1x1 conv_shortcut over the concat is split into its two column blocks.  UAV_VIRTUAL_CONCAT=0 disables it.
-VIRTUAL_CONCAT = os.environ.get("UAV_VIRTUAL_CONCAT", "1") != "0"
-
-
+# 1x1 conv_shortcut over the concat is split into its two column blocks.
 def new_cat_slot(skip, cx: int, batch: int, producer_has_stats: bool = False):
     """-> the head slice (batch, t, h, w, cx) of a fresh concat buffer whose tail already holds `skip`; the producer of
     the main branch writes into it and `cat_with_skip` later returns the whole buffer.  None (plain allocation by the
     producer) when the concat will not be materialised at all."""
-    if not INPLACE_CONCAT:
-        return None
-    if VIRTUAL_CONCAT and ops.GN_FUSED_STATS and producer_has_stats and getattr(skip, "uav_gn", None):
+    if producer_has_stats and getattr(skip, "uav_gn", None):
         return None
     cs = skip.shape[-1]
     buf = torch.empty(batch, *skip.shape[1:-1], cx + cs, dtype=skip.dtype, device=skip.device)
@@ -302,7 +270,7 @@ class ResnetBlock3D(nn.Module):
         """forward(torch.cat([x, skip], channel)) (unet_blocks.py:573,645) without building the concatenation when both
         tensors carry their producers' GroupNorm statistics; otherwise through the (in-place) concat buffer"""
         h = None
-        if (VIRTUAL_CONCAT and self.conv_shortcut is not None and isinstance(self.conv_shortcut, InflatedConv3d)
+        if (self.conv_shortcut is not None and isinstance(self.conv_shortcut, InflatedConv3d)
                 and getattr(x, "uav_cat", None) is None):
             g, b = c.pk.affine(self.norm1)
             h = ops.group_norm_cat([x, skip], g, b, self.norm1.num_groups, self.norm1.eps, silu=True, n_outer=x.shape[0])
@@ -398,7 +366,7 @@ class Upsample3D(nn.Module):
     def forward(self, c: Ctx, x, output_size=None, stream_scale: float = 1.0, out=None):
         assert x.shape[-1] == self.channels
         exact2x = output_size is None or tuple(output_size[-2:]) == (2 * x.shape[-3], 2 * x.shape[-2])
-        if (self.conv is not None and exact2x and FUSE_UPSAMPLE_CONV and self.out_channels >= 64
+        if (self.conv is not None and exact2x and self.out_channels >= 64
                 and self.out_channels % 8 == 0 and self.channels % 8 == 0):
             # nearest x2 + 3x3 conv as four 2x2 phase convs on the source (4/9 of the MACs, no 4x intermediate)
             w4 = c.pk.tensor(f"up4_{id(self.conv)}",
@@ -445,8 +413,7 @@ class CrossAttention(nn.Module):
         self.to_out = nn.ModuleList([nn.Linear(inner, query_dim), nn.Dropout(0.0)])
 
     def forward(self, c: Ctx, norm, hs, frames: int):
-        """hs: residual stream (B, T, HW, C); returns to_out(attn(LayerNorm(hs))) + hs.  The LayerNorm rides the q (or
-        q|k|v) projection's epilogue when hs carries its producer's row statistics (ops.LnStats)."""
+        """hs: residual stream (B, T, HW, C); returns to_out(attn(LayerNorm(hs))) + hs."""
         B, T, HW, C = hs.shape
         if self.is_cross:
             q = _ln_linear(c, norm, [self.to_q], f"lnq{id(self)}", hs).view(B * T, HW, C)
@@ -458,19 +425,14 @@ class CrossAttention(nn.Module):
             qkv = _ln_linear(c, norm, [self.to_q, self.to_k, self.to_v], f"lnqkv{id(self)}", hs).view(B * T, HW, 3 * C)
             o = ops.attention(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], self.heads)
         wo, bo = c.pk.linear(self.to_out[0])
-        return ops.linear(o.view(B, T, HW, C), wo, bo, residual=hs, ln_stats=True)
+        return ops.linear(o.view(B, T, HW, C), wo, bo, residual=hs)
 
 
 def _ln_linear(c: Ctx, norm: nn.LayerNorm, mods, key: str, hs, **kw):
-    """Linear(s) `mods` applied to LayerNorm(hs): folded into one GEMM when hs carries row statistics, else LayerNorm
-    kernel + GEMM on the fused weights"""
-    st = getattr(hs, "uav_ln", None)
-    if st is not None and ops.LN_FUSED and st.C == hs.shape[-1]:
-        w, b, colsum = c.pk.ln_linear(key, norm, mods)
-        return ops.linear(hs, w, b, ln=(st, colsum, norm.eps), **kw)
+    """Linear(s) `mods` applied to LayerNorm(hs): LayerNorm kernel + one GEMM on the row-concatenated weights"""
     g, bt = c.pk.affine(norm)
     n = ops.layer_norm(hs, g, bt, norm.eps)
-    w, b = c.pk.fused_linear(key + "_plain", mods) if len(mods) > 1 else c.pk.linear(mods[0])
+    w, b = c.pk.fused_linear(key, mods) if len(mods) > 1 else c.pk.linear(mods[0])
     return ops.linear(n, w, b, **kw)
 
 
@@ -528,7 +490,7 @@ class TemporalAttention(CrossAttention):
         bias = c.pk.tensor(f"relbias{id(self)}_{T}", lambda: self.time_rel_pos_bias.table(T))
         o = ops.temporal_attention(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], self.heads, c.rot, bias)
         wo, bo = c.pk.linear(self.to_out[0])
-        return ops.linear(o, wo, bo, residual=hs, ln_stats=True)
+        return ops.linear(o, wo, bo, residual=hs)
 
 
 class GEGLU(nn.Module):
@@ -608,12 +570,12 @@ class Transformer3DModel(nn.Module):
         x = self.resblock_temporal(c, x)
         hs = _gn(c, self.norm, x, False, B * T)
         w, b = c.pk.linear(self.proj_in)
-        hs = ops.linear(hs.view(B, T, H * W, C), w, b, ln_stats=True)
+        hs = ops.linear(hs.view(B, T, H * W, C), w, b)
         for blk in self.transformer_blocks:
             hs = blk(c, hs)
         w, b = c.pk.linear(self.proj_out)
         dst = None if out is None else out.view(B, T, H * W, C)
-        y = ops.linear(hs, w, b, residual=x.view(B, T, H * W, C), gn_stats=GN_STATS_LINEAR, out=dst)
+        y = ops.linear(hs, w, b, residual=x.view(B, T, H * W, C), gn_stats=True, out=dst)
         if out is not None:
             return _carry_gn(out, y)
         return _carry_gn(y.view(B, T, H, W, C), y)
@@ -640,7 +602,7 @@ class TemporalModule3D(nn.Module):
     def forward(self, c: Ctx, x, out=None):
         h = self.resblocks_3d_temporal(c, x)
         h = self.resblocks_3d_spatial(c, h)
-        return self.shift_conv.run(c, h, residual=x, gn_stats=GN_STATS_LINEAR, out=out)
+        return self.shift_conv.run(c, h, residual=x, gn_stats=True, out=out)
 
 
 class EmptyTemporalModule3D(nn.Module):
@@ -747,7 +709,7 @@ class UpBlock3D(nn.Module):
             # the main branch of the next concat is produced by this stage's last layer: let it store there directly
             # (unless that concat will not be materialised at all: both halves carry GroupNorm statistics)
             nxt = (out if self.upsamplers is None else None) if last else \
-                new_cat_slot(skips[-2 - i], r.out_channels, B, GN_STATS_LINEAR if self.attentions is not None else True)
+                new_cat_slot(skips[-2 - i], r.out_channels, B, True)
             if self.attentions is not None:
                 x = r.forward_cat(c, x, skips[-1 - i])
                 x = self.attentions[i](c, x, out=nxt)
@@ -799,7 +761,7 @@ class AttentionBlock(nn.Module):
                           scale=(C // self.num_heads) ** -0.5)
         wo, bo = c.pk.linear(self.proj_attn)
         out = ops.linear(o.view(B, T, H * W, C), wo, bo, residual=x.view(B, T, H * W, C), out_scale=stream_scale,
-                         gn_stats=GN_STATS_LINEAR)
+                         gn_stats=True)
         return _carry_gn(out.view(B, T, H, W, C), out)
 
 

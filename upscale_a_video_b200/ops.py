@@ -133,28 +133,9 @@ class GnStats:
         return 0
 
 
-class LnStats:
-    """per-row {sum, sumsq} slots of a token tensor, written by the epilogue of the Linear that produced it
-    (uav_epilogue_t.ln_out): fp32 [rows][slots][2]; attached as `tensor.uav_ln`.  The Linear that consumes
-    LayerNorm(tensor) folds the normalisation into its epilogue (uav_epilogue_t.ln_in)."""
-    __slots__ = ("partial", "slots", "C")
-
-    def __init__(self, partial, slots, C):
-        self.partial, self.slots, self.C = partial, slots, C
-
-
-GN_FUSED_STATS = __import__("os").environ.get("UAV_GN_FUSED_STATS", "1") != "0"
-# LayerNorm folded into the consuming Linear (uav_epilogue_t.ln_in / ln_out).  OFF by default: the short-K Linears that
-# consume a LayerNorm have their epilogue on the critical path, and the fold moves them from the lean bias-only kernel
-# instance to the AUX one (+ row-statistics loads, + column-sum loads, + 2 FMA per element on the producers), which cost
-# more than the LayerNorm passes it removes.  Not re-measured on H100.  Kept as an opt-in (UAV_LN_FUSED=1) with its
-# parity test.
-LN_FUSED = __import__("os").environ.get("UAV_LN_FUSED", "0") == "1"
-
-
 def _gn_request(out: torch.Tensor, n_out: int, w: int, h: int, images: int, batch: int, e: Epilogue):
     """arm the epilogue to emit the statistics blocks of `out`; returns the GnStats to attach after the launch"""
-    if not GN_FUSED_STATS or out.dtype != torch.float16 or n_out < 64 or n_out % 8:
+    if out.dtype != torch.float16 or n_out < 64 or n_out % 8:
         return None
     blocks = int(_lib.load().uav_gn_partial_blocks(w, h, images))
     partial = torch.empty(n_out // 8, blocks, 2, dtype=torch.float32, device=out.device)
@@ -187,11 +168,8 @@ def _epi(out: torch.Tensor, bias=None, rowvec=None, rows_per_vec=0, residual=Non
 
 def linear(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, *, out=None,
            residual=None, rowvec=None, rows_per_vec=0, act=ACT_NONE, out_dtype=torch.float16, out_scale=1.0,
-           gn_stats=False, ln=None, ln_stats=False):
-    """out[..., N] = epilogue(a[..., K] @ w[N, K]^T); a fp16 (rows may be a channel-slice view).
-    `ln=(LnStats of a, colsum fp32 [N], eps)`: the result is LayerNorm(a) @ W^T + b with w = W * gamma, bias = b + W beta
-    pre-packed by the caller (layers.Packed.ln_linear) — the normalised tensor is never materialised.
-    `ln_stats`: emit the row statistics of the OUTPUT (`out.uav_ln`) for the LayerNorm that follows."""
+           gn_stats=False):
+    """out[..., N] = epilogue(a[..., K] @ w[N, K]^T); a fp16 (rows may be a channel-slice view)."""
     assert a.dtype == torch.float16 and w.dtype == torch.float16 and w.is_contiguous()
     K = a.shape[-1]
     N = w.shape[0]
@@ -204,22 +182,11 @@ def linear(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None
     e = _epi(out, bias, rowvec, rows_per_vec, residual, act, out_scale)
     st = _gn_request(out, n_out, M, 1, 1, a.shape[0] if a.dim() > 2 else 1, e) if gn_stats and act != ACT_GEGLU else None
     lib = _lib.load()
-    if ln is not None:
-        lst, colsum, eps = ln
-        assert lst.C == K and lst.partial.shape[0] == M and colsum.dtype == torch.float32 and colsum.numel() == N
-        e.ln_in, e.ln_colsum, e.ln_slots, e.ln_eps = lst.partial.data_ptr(), colsum.data_ptr(), lst.slots, eps
-    lo = None
-    if ln_stats and LN_FUSED and act != ACT_GEGLU and out.dtype == torch.float16 and n_out >= 64 and n_out % 8 == 0:
-        slots = int(lib.uav_ln_partial_slots(n_out))
-        lo = LnStats(torch.empty(M, slots, 2, dtype=torch.float32, device=out.device), slots, n_out)
-        e.ln_out, e.ln_out_slots = lo.partial.data_ptr(), slots
     with _timed("igemm", 2.0 * M * N * K, 2.0 * (M * K + N * K + M * n_out), f"linear M{M} K{K} N{N} act{act}"):
         _lib.check(lib.uav_linear(a.data_ptr(), M, K, _pixel_ld(a) if a.dim() > 1 else K, w.data_ptr(), N,
                                   out.data_ptr(), C.byref(e), _stream()), "uav_linear")
     if st is not None:
         out.uav_gn = [st]
-    if lo is not None:
-        out.uav_ln = lo
     return out
 
 
@@ -421,7 +388,7 @@ def group_norm_cat(parts, gamma: torch.Tensor, beta: torch.Tensor, groups: int, 
 def _gn_sources(x, stats, groups: int, n_outer: int, batch: int):
     """ctypes source table for a tensor whose producer(s) emitted GroupNorm statistics, or None"""
     C = x.shape[-1]
-    if not (GN_FUSED_STATS and stats and (C // groups) % 8 == 0 and len(stats) <= 4 and sum(s.C for s in stats) == C):
+    if not (stats and (C // groups) % 8 == 0 and len(stats) <= 4 and sum(s.C for s in stats) == C):
         return None
     slabs = [s.slabs_for(n_outer, batch) for s in stats]
     if not all(slabs):
@@ -700,7 +667,11 @@ def add_noise(x, noise, sqrt_alpha: float, sqrt_one_minus_alpha: float):
 
 def propagate_step(feat_prop, feat_cur, flow_prop, flow_check, out, *, nearest: bool, fuse: bool, fuse_scale: float,
                    alpha1: float, alpha2: float, half_grid_sample: bool):
-    """all tensors are (C|2, H, W) views with contiguous planes (stride(-1)==1, stride(-2)==W)"""
+    """all tensors are (C|2, H, W) views with contiguous planes (stride(-1)==1, stride(-2)==W).
+    `half_grid_sample`: how the grid sample rounds half inputs.  Only False is implemented: the opmath form of torch's
+    CUDA grid_sampler (fp32 coordinates and weights, one final rounding); True raises."""
+    if half_grid_sample:
+        raise _lib.UavError("propagate_step: only the opmath grid sample (half_grid_sample=False) is implemented")
     Cc, H, W = feat_prop.shape
     for t in (feat_prop, feat_cur, flow_prop, flow_check, out):
         assert t.stride(-1) == 1 and t.stride(-2) == W and t.dtype == feat_prop.dtype and t.is_cuda
@@ -710,7 +681,7 @@ def propagate_step(feat_prop, feat_cur, flow_prop, flow_check, out, *, nearest: 
                                       flow_check.data_ptr(), out.data_ptr(), Cc, H, W, feat_prop.stride(0),
                                       feat_cur.stride(0), out.stride(0), flow_prop.stride(0), flow_check.stride(0),
                                       1 if nearest else 0, 1 if fuse else 0, fuse_scale, alpha1, alpha2,
-                                      1 if half_grid_sample else 0, dt, _stream()), "uav_propagate_step")
+                                      dt, _stream()), "uav_propagate_step")
     return out
 
 

@@ -8,17 +8,12 @@ rounding sequence (SURVEY.md fact 8: coordinates are fp16, nearest sampling).  T
 inherently sequential (each warp reads arbitrary pixels of the previous result), so there are 2*(T-1) launches."""
 from __future__ import annotations
 
-import os
-
 import torch
 from torch import nn
 
 from . import ops
 from . import _lib
 from ._lib import UavError
-
-# How torch's CUDA grid_sampler treats fp16 inputs (see csrc/sampler.cu): 0 = opmath/fp32 intermediates.
-HALF_GRID_SAMPLE = int(os.environ.get("UAV_HALF_GRID_SAMPLE", "0"))
 
 
 class Propagation(nn.Module):
@@ -68,7 +63,7 @@ class Propagation(nn.Module):
                                            f_check[bi, :, flow_idx[i]], out[bi, :, idx],
                                            nearest=(interpolation == "nearest"), fuse=(mode == "fuse"),
                                            fuse_scale=float(fuse_scale), alpha1=float(alpha1), alpha2=float(alpha2),
-                                           half_grid_sample=bool(HALF_GRID_SAMPLE))
+                                           half_grid_sample=False)
                     prev = idx
             cur = out
         return cur

@@ -29,7 +29,6 @@ from ._lib import UavError
 from .layers import (CrossAttention, CrossAttnDownBlock3D, CrossAttnUpBlock3D, Ctx, DownBlock3D, EmptyTemporalModule3D,
                      InflatedConv3d, PackedModule, ResnetBlock3D, RotaryEmbedding, TemporalModule3D,
                      UNetMidBlock3DCrossAttn, UpBlock3D, _gn, new_cat_slot)
-from . import layers as _layers
 
 
 @dataclass
@@ -55,12 +54,6 @@ class TimestepEmbedding(nn.Module):
         self.linear_1 = nn.Linear(in_channels, time_embed_dim)
         self.linear_2 = nn.Linear(time_embed_dim, time_embed_dim)
 
-
-# compute the text-independent UNet prefix once for both classifier-free-guidance halves (UAV_SHARE_CFG_PREFIX=0: off)
-SHARE_CFG_PREFIX = os.environ.get("UAV_SHARE_CFG_PREFIX", "1") != "0"
-
-# conv_norm_out + SiLU + conv_out + layout conversion as one kernel (csrc/conv_io.cu); UAV_FUSED_CONV_OUT=0: separate kernels
-FUSED_CONV_OUT = os.environ.get("UAV_FUSED_CONV_OUT", "1") != "0"
 
 _DOWN = {"DownBlock3D": DownBlock3D, "CrossAttnDownBlock3D": CrossAttnDownBlock3D}
 _UP = {"UpBlock3D": UpBlock3D, "CrossAttnUpBlock3D": CrossAttnUpBlock3D}
@@ -230,7 +223,7 @@ class UNetVideoModel(PackedModule, ConfigMixin):
         `cfg_step` (keyword-only extension, set by VideoUpscalePipeline for the single-window case): dict(guidance_scale,
         pred_type, sqrt_alpha, sqrt_beta, clip, clip_range, sample) — classifier-free guidance and DDIMScheduler.step_v0
         (pipeline...:644-649) run in conv_out's epilogue and a UNetCfgStepOutput is returned; ignored (plain output) when
-        the fused tail does not apply (batch != 2, fp32 working dtype, UAV_FUSED_CONV_OUT=0)."""
+        the fused tail does not apply (batch != 2, fp32 working dtype)."""
         _lib.require_cuda(sample, "UNetVideoModel.forward")
         if attention_mask is not None:
             raise NotImplementedError("attention_mask is never passed by VideoUpscalePipeline")
@@ -248,7 +241,7 @@ class UNetVideoModel(PackedModule, ConfigMixin):
         if cin != cfg.in_channels:
             raise ValueError(f"expected {cfg.in_channels} input channels, got {cin}")
         share = (cfg_shared_input and B == 2 and len(self.down_blocks) > 1 and not self.down_blocks[0].has_cross_attention
-                 and self.down_blocks[1].has_cross_attention and SHARE_CFG_PREFIX)
+                 and self.down_blocks[1].has_cross_attention)
         Bp = 1 if share else B
         x = torch.zeros(Bp, T, H, W, (cin + 7) // 8 * 8, dtype=torch.float16, device=dev)
         ops.planar_to_channels_last(sample[:Bp].contiguous(), x, 0)
@@ -305,7 +298,7 @@ class UNetVideoModel(PackedModule, ConfigMixin):
 
         mid_empty = isinstance(self.mid_temp_block, EmptyTemporalModule3D)
         c_mid = cfg.block_out_channels[-1]
-        slot = first_slot(0, c_mid, x.shape[2:4], True if mid_empty else _layers.GN_STATS_LINEAR)
+        slot = first_slot(0, c_mid, x.shape[2:4], True)
         x = self.mid_block(c, x, out=slot if mid_empty else None)
         _tap("mid", x)
         x = self.mid_temp_block(c, x, out=None if mid_empty else slot)
@@ -319,16 +312,15 @@ class UNetVideoModel(PackedModule, ConfigMixin):
             slot = None
             if not final:
                 hw = tuple(up_size[1:]) if up_size is not None else (2 * x.shape[2], 2 * x.shape[3])
-                # producer of the next block's main branch: the temporal module's shift_conv (statistics if Linear producers
-                # emit them) or, without a temporal module, the upsampler conv (its four phase launches emit none)
-                slot = first_slot(i + 1, blk.resnets[-1].out_channels, hw,
-                                  False if t_empty else _layers.GN_STATS_LINEAR)
+                # producer of the next block's main branch: the temporal module's shift_conv (emits statistics) or,
+                # without a temporal module, the upsampler conv (its four phase launches emit none)
+                slot = first_slot(i + 1, blk.resnets[-1].out_channels, hw, not t_empty)
             x = blk(c, x, res, up_size, out=slot if t_empty else None)
             _tap(f"up{i}", x)
             x = tmod(c, x, out=None if t_empty else slot)
             _tap(f"up_temp{i}", x)
         out_dtype = sample.dtype if sample.dtype in (torch.float16, torch.float32) else torch.float16
-        if FUSED_CONV_OUT and x.shape[-1] == 256 and cfg.out_channels <= 5 and x.shape[0] == B:
+        if x.shape[-1] == 256 and cfg.out_channels <= 5 and x.shape[0] == B:
             # GroupNorm apply + SiLU + conv_out + the rearrange to "b c t h w" in ONE pass over the 256-channel tensor
             g, bt = c.pk.affine(self.conv_norm_out)
             w, bias = c.pk.conv(self.conv_out)
