@@ -1,5 +1,6 @@
-"""per-shape timing of one UNet forward at config 2 (B=2 = the two CFG halves of one clip, T=8, 320x576), as the pipeline
-calls it (cfg_shared_input=True)"""
+"""per-shape timing of one UNet forward (B=2 = the two CFG halves of one clip, T=8) as the pipeline calls it
+(cfg_shared_input=True): --config c2 (320x576, the default) or h720 (180x320, the clip bench.py times by default)"""
+import argparse
 import json
 import os
 import sys
@@ -9,13 +10,18 @@ import torch
 from upscale_a_video_b200 import UNetVideoModel, ops
 from upscale_a_video_b200.synthetic import seeded_state_dict
 
+SIZES = {"c2": (320, 576), "h720": (180, 320)}
+ap = argparse.ArgumentParser()
+ap.add_argument("--config", default="c2", choices=sorted(SIZES))
+H, W = SIZES[ap.parse_args().config]
+
 dev = torch.device("cuda")
 cfg = json.load(open(os.path.join(os.path.dirname(__file__), "..", "upscale_a_video_b200", "configs", "unet_video_config.json")))
 unet = UNetVideoModel.from_config(cfg)
 unet.load_state_dict(seeded_state_dict(unet, 1234))
 unet = unet.half().eval().to(dev)
-lat = torch.randn(1, 4, 8, 320, 576, device=dev, dtype=torch.float16).repeat(2, 1, 1, 1, 1)
-low = torch.randn(1, 3, 8, 320, 576, device=dev, dtype=torch.float16).repeat(2, 1, 1, 1, 1)
+lat = torch.randn(1, 4, 8, H, W, device=dev, dtype=torch.float16).repeat(2, 1, 1, 1, 1)
+low = torch.randn(1, 3, 8, H, W, device=dev, dtype=torch.float16).repeat(2, 1, 1, 1, 1)
 ctx = (torch.randn(2, 77, 1024, device=dev) * 0.3).half()
 kw = dict(encoder_hidden_states=ctx, class_labels=torch.tensor([120]), cfg_shared_input=True)
 

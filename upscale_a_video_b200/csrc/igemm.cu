@@ -13,6 +13,9 @@
 //    wgmma m64 x BLOCK_N x 16 on their 64 rows of the stage and run the fused epilogue from the register accumulators
 //    (bias/temb/act/residual/statistics -> swizzled smem staging -> TMA store); an mbarrier ring of {A 128x64,
 //    B BLOCK_Nx64} fp16 stages fills the rest of the 227 KB of shared memory.
+//  * tiles are 128 x BLOCK_N with BLOCK_N up to 256: the producer warpgroup gives up registers (setmaxnreg.dec 40) so
+//    that each consumer thread can hold the 128 fp32 accumulators of an m64n256 tile (setmaxnreg.inc 232).  A 256-wide
+//    tile fetches every A box once per 256 output channels instead of once per 128.
 //  * stride-2 convs read a 5-D "phase" view (2C, W/2, 2, H/2, NB) of the same buffer, the
 //    temporal (k,1,1) conv a (C, HW, T, B) view, Conv3d a (C, W, H, T, B) view, Linear a
 //    (K, M) view: all the same kernel, only the tensor map and the tap table differ.
@@ -127,6 +130,7 @@ struct IgemmCfg {
   static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + AUX_BYTES + 1024 /*align*/;
   static constexpr int ACC = BLOCK_N / 2;  // fp32 accumulator registers per thread: m64 x BLOCK_N per warpgroup
+  static_assert(SMEM_BYTES <= SMEM_LIMIT, "stage ring + output staging exceed the shared memory of a block");
 };
 
 __device__ __forceinline__ void epi_bar_sync() {
@@ -195,6 +199,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
 
   if (warp_idx < 4) {
     // =============================== TMA producer ===============================
+    // 128 x 40 + 256 x 232 registers fit the 64 K register file
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -238,6 +244,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
   }
 
   // =============================== wgmma consumers + epilogue ===============================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
   const int et = threadIdx.x - 128;  // 0..255
   const int wg = et >> 7;            // rows [64 wg, +64) of the tile
   const int cw = et >> 5;            // rows [16 cw, +16): the accumulator rows of this warp
@@ -341,87 +348,98 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
         }
       }
     }
+    // The epilogue runs in passes of at most 128 columns over acc[0, EPI_ACC), shifting the next columns down after
+    // each pass: an unrolled 256-column AUX epilogue would be twice the code and no longer fit the instruction cache.
+    constexpr int EPI_N = GEGLU ? OUT_TILE_N : (OUT_TILE_N < 128 ? OUT_TILE_N : 128);
+    constexpr int EPI_ACC = EPI_N / 2;
+#pragma unroll 1
+    for (int pass = 0; pass < OUT_TILE_N / EPI_N; ++pass) {
 #pragma unroll
-    for (int jb = 0; jb < OUT_TILE_N / 8; ++jb) {
-      const int col = jb * 8 + 2 * lr;  // column inside the output tile (this thread: col, col + 1)
-      const int n = n_base + col;
-      const bool ok0 = n < p.n_out, ok1 = n + 1 < p.n_out;
-      float b0 = 0.f, b1 = 0.f, g0 = 0.f, g1 = 0.f;
-      if (p.bias != nullptr) {
-        if (ok0) b0 = __ldg(p.bias + n);
-        if (ok1) b1 = __ldg(p.bias + n + 1);
-        if (GEGLU) {
-          if (ok0) g0 = __ldg(p.bias + p.N / 2 + n);
-          if (ok1) g1 = __ldg(p.bias + p.N / 2 + n + 1);
+      for (int jb = 0; jb < EPI_N / 8; ++jb) {
+        const int col = pass * EPI_N + jb * 8 + 2 * lr;  // column inside the output tile (this thread: col, col + 1)
+        const int n = n_base + col;
+        const bool ok0 = n < p.n_out, ok1 = n + 1 < p.n_out;
+        float b0 = 0.f, b1 = 0.f, g0 = 0.f, g1 = 0.f;
+        if (p.bias != nullptr) {
+          if (ok0) b0 = __ldg(p.bias + n);
+          if (ok1) b1 = __ldg(p.bias + n + 1);
+          if (GEGLU) {
+            if (ok0) g0 = __ldg(p.bias + p.N / 2 + n);
+            if (ok1) g1 = __ldg(p.bias + p.N / 2 + n + 1);
+          }
         }
-      }
-      float gs = 0.f, gq = 0.f;  // GroupNorm statistics of this 8-column group over the thread's rows
+        float gs = 0.f, gq = 0.f;  // GroupNorm statistics of this 8-column group over the thread's rows
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const float a0 = acc[4 * jb + 2 * h], a1 = acc[4 * jb + 2 * h + 1];
-        float x0, x1;
-        if constexpr (GEGLU) {
-          constexpr int GJ = OUT_TILE_N / 8;  // gate columns start at accumulator column OUT_TILE_N
-          const float q0 = acc[4 * (jb + GJ) + 2 * h], q1 = acc[4 * (jb + GJ) + 2 * h + 1];
-          x0 = (a0 + b0) * gelu_erf_f(q0 + g0);
-          x1 = (a1 + b1) * gelu_erf_f(q1 + g1);
-        } else {
-          x0 = a0 + b0;
-          x1 = a1 + b1;
-        }
-        // staging address of (row, col): 16-byte chunk (col & 63) / 8 of the row, CU_TENSOR_MAP_SWIZZLE_128B
-        const uint32_t row = lrow[h];
-        uint8_t* sp = staging + (col >> 6) * SLAB_BYTES + row * 128 + ((((col & 63) >> 3) ^ (row & 7)) << 4) + (col & 7) * 2;
-        if constexpr (AUX) {
-          if (rv[h] != nullptr) {
-            if (ok0) x0 += __half2float(rv[h][n]);
-            if (ok1) x1 += __half2float(rv[h][n + 1]);
-          }
-          if (p.act != UAV_ACT_NONE) {
-            x0 = apply_act(x0, p.act);
-            x1 = apply_act(x1, p.act);
-          }
-          if (TMA_EPI && p.res_tma) {  // residual of this row from the staging tile (same swizzle as the store)
-            const float2 r = __half22float2(*reinterpret_cast<const __half2*>(sp));
-            x0 = fmaf(x0, p.out_scale, r.x);
-            x1 = fmaf(x1, p.out_scale, r.y);
-          } else if (res[h] != nullptr) {
-            x0 = fmaf(x0, p.out_scale, ok0 ? __half2float(res[h][n]) : 0.f);
-            x1 = fmaf(x1, p.out_scale, ok1 ? __half2float(res[h][n + 1]) : 0.f);
-          } else if (p.out_scale != 1.0f) {
-            x0 *= p.out_scale;
-            x1 *= p.out_scale;
-          }
-          if (row_ok[h] && ok0) {
-            gs += x0 + x1;
-            gq = fmaf(x0, x0, fmaf(x1, x1, gq));
-          }
-        }
-        if constexpr (TMA_EPI) {
-          *reinterpret_cast<uint32_t*>(sp) = pack_half2_sat(x0, x1);
-        } else if (row_ok[h]) {
-          if (p.out_dtype == UAV_F16) {
-            __half* op = reinterpret_cast<__half*>(p.out) + out_row[h] * p.ld_out + n;
-            if (ok0) op[0] = __float2half_rn(fminf(fmaxf(x0, -65504.f), 65504.f));
-            if (ok1) op[1] = __float2half_rn(fminf(fmaxf(x1, -65504.f), 65504.f));
+        for (int h = 0; h < 2; ++h) {
+          const float a0 = acc[4 * jb + 2 * h], a1 = acc[4 * jb + 2 * h + 1];
+          float x0, x1;
+          if constexpr (GEGLU) {
+            constexpr int GJ = OUT_TILE_N / 8;  // gate columns start at accumulator column OUT_TILE_N
+            const float q0 = acc[4 * (jb + GJ) + 2 * h], q1 = acc[4 * (jb + GJ) + 2 * h + 1];
+            x0 = (a0 + b0) * gelu_erf_f(q0 + g0);
+            x1 = (a1 + b1) * gelu_erf_f(q1 + g1);
           } else {
-            float* op = reinterpret_cast<float*>(p.out) + out_row[h] * p.ld_out + n;
-            if (ok0) op[0] = x0;
-            if (ok1) op[1] = x1;
+            x0 = a0 + b0;
+            x1 = a1 + b1;
+          }
+          // staging address of (row, col): 16-byte chunk (col & 63) / 8 of the row, CU_TENSOR_MAP_SWIZZLE_128B
+          const uint32_t row = lrow[h];
+          uint8_t* sp = staging + (col >> 6) * SLAB_BYTES + row * 128 + ((((col & 63) >> 3) ^ (row & 7)) << 4) + (col & 7) * 2;
+          if constexpr (AUX) {
+            if (rv[h] != nullptr) {
+              if (ok0) x0 += __half2float(rv[h][n]);
+              if (ok1) x1 += __half2float(rv[h][n + 1]);
+            }
+            if (p.act != UAV_ACT_NONE) {
+              x0 = apply_act(x0, p.act);
+              x1 = apply_act(x1, p.act);
+            }
+            if (TMA_EPI && p.res_tma) {  // residual of this row from the staging tile (same swizzle as the store)
+              const float2 r = __half22float2(*reinterpret_cast<const __half2*>(sp));
+              x0 = fmaf(x0, p.out_scale, r.x);
+              x1 = fmaf(x1, p.out_scale, r.y);
+            } else if (res[h] != nullptr) {
+              x0 = fmaf(x0, p.out_scale, ok0 ? __half2float(res[h][n]) : 0.f);
+              x1 = fmaf(x1, p.out_scale, ok1 ? __half2float(res[h][n + 1]) : 0.f);
+            } else if (p.out_scale != 1.0f) {
+              x0 *= p.out_scale;
+              x1 *= p.out_scale;
+            }
+            if (row_ok[h] && ok0) {
+              gs += x0 + x1;
+              gq = fmaf(x0, x0, fmaf(x1, x1, gq));
+            }
+          }
+          if constexpr (TMA_EPI) {
+            *reinterpret_cast<uint32_t*>(sp) = pack_half2_sat(x0, x1);
+          } else if (row_ok[h]) {
+            if (p.out_dtype == UAV_F16) {
+              __half* op = reinterpret_cast<__half*>(p.out) + out_row[h] * p.ld_out + n;
+              if (ok0) op[0] = __float2half_rn(fminf(fmaxf(x0, -65504.f), 65504.f));
+              if (ok1) op[1] = __float2half_rn(fminf(fmaxf(x1, -65504.f), 65504.f));
+            } else {
+              float* op = reinterpret_cast<float*>(p.out) + out_row[h] * p.ld_out + n;
+              if (ok0) op[0] = x0;
+              if (ok1) op[1] = x1;
+            }
+          }
+        }
+        if constexpr (AUX && TMA_EPI) {
+          if (p.gn_partial != nullptr) {  // warp-uniform: the 16 rows x 8 columns of this warp
+            gs = warp_sum(gs);
+            gq = warp_sum(gq);
+            const int oct = n >> 3;
+            const int64_t blk = static_cast<int64_t>(m_tile) * 8 + cw;
+            if (lane == 0 && blk < p.gn_blocks && oct * 8 < p.n_out) {
+              p.gn_partial[(static_cast<int64_t>(oct) * p.gn_blocks + blk) * 2] = gs;
+              p.gn_partial[(static_cast<int64_t>(oct) * p.gn_blocks + blk) * 2 + 1] = gq;
+            }
           }
         }
       }
-      if constexpr (AUX && TMA_EPI) {
-        if (p.gn_partial != nullptr) {  // warp-uniform: the 16 rows x 8 columns of this warp
-          gs = warp_sum(gs);
-          gq = warp_sum(gq);
-          const int oct = (n_base >> 3) + jb;
-          const int64_t blk = static_cast<int64_t>(m_tile) * 8 + cw;
-          if (lane == 0 && blk < p.gn_blocks && oct * 8 < p.n_out) {
-            p.gn_partial[(static_cast<int64_t>(oct) * p.gn_blocks + blk) * 2] = gs;
-            p.gn_partial[(static_cast<int64_t>(oct) * p.gn_blocks + blk) * 2 + 1] = gq;
-          }
-        }
+      if (pass + 1 < OUT_TILE_N / EPI_N) {
+#pragma unroll
+        for (int i = 0; i + EPI_ACC < Cfg::ACC; ++i) acc[i] = acc[i + EPI_ACC];
       }
     }
     if constexpr (TMA_EPI) {
@@ -499,6 +517,23 @@ static uav_status_t launch_instance(IgemmParams& p, cudaStream_t stream) {
   return launch_instance2<BLOCK_N, GEGLU, false, true>(p, stream);
 }
 
+// Time of one 256-column tile over one 128-column tile of the same GEMM (GEGLU: 128 over 64 output columns), from
+// tools/bench_igemm.py on an H100 80GB HBM3 at 700 W.  On launches of many waves (twice the ratio of the kernel times at
+// the two widths) 3x3 convs give 1.46 to 1.62, the (3,1,1) temporal conv 1.55 and GEGLU 512->4096 1.69 and 1.90.  Launches
+// of few waves gain less: the h720 convs 512->512 on 16 x 45x80 (8 wide against 15 narrow waves) and 1024->1024 on
+// 16 x 23x40 (5 against 9) took 0.47 and 0.56 ms with 256-column tiles against 0.41 and 0.49 ms with 128-column tiles.
+// 1.9 keeps both of those at 128 columns and still takes the wide tiles for the GEGLU and the many-wave convolutions.
+constexpr double WIDE_TILE_COST = 1.9;
+
+// A persistent launch takes ceil(tiles / SMs) waves; the wide tiles win when their fewer waves, each WIDE_TILE_COST times
+// as long, finish before the narrow ones.  out_wide = output columns of a wide tile.
+static bool wide_tile_pays(uint64_t m_tiles, int64_t n_out, int64_t out_wide) {
+  const uint64_t sms = (uint64_t)num_sms();
+  const uint64_t waves_wide = (m_tiles * ((n_out + out_wide - 1) / out_wide) + sms - 1) / sms;
+  const uint64_t waves_narrow = (m_tiles * ((2 * n_out + out_wide - 1) / out_wide) + sms - 1) / sms;
+  return (double)waves_wide * WIDE_TILE_COST < (double)waves_narrow;
+}
+
 static uav_status_t launch_igemm(const IgemmDesc& d, cudaStream_t stream) {
   const uav_epilogue_t* e = d.epi;
   UAV_REQUIRE(e != nullptr, "igemm: epilogue descriptor is NULL");
@@ -516,9 +551,17 @@ static uav_status_t launch_igemm(const IgemmDesc& d, cudaStream_t stream) {
 
   IgemmParams p;
   memset(&p, 0, sizeof(p));
-  // 128-column tiles at most: two m64 x 128 fp32 accumulators (64 registers per thread) per CTA
+  uint64_t m_tiles = 1;
+  for (int i = 1; i < 5; ++i) m_tiles *= d.tiles[i];
+  // 256-column tiles (128 output columns with GEGLU) for convolutions and GEGLU with N >= 256, unless they lose to wave
+  // quantisation; 128-column tiles for the rest of N > 64.  Single-tap GEMMs without GEGLU (Linear, 1x1 conv) keep
+  // 128-column tiles: their short main loop does not hide the twice as long epilogue of a 256-column tile (measured: no
+  // gain at K = 2048, 10% slower at K = 512).  GEGLU-256 needs N % 256 == 0 so that the value box never reads gate rows.
+  const int64_t n_out = geglu ? d.N / 2 : d.N;
   int block_n;
-  if (geglu || d.N > 64) block_n = 128;
+  if (geglu) block_n = (d.N % 256 == 0 && wide_tile_pays(m_tiles, n_out, 128)) ? 256 : 128;
+  else if (d.N >= 256 && d.num_taps > 1 && wide_tile_pays(m_tiles, n_out, 256)) block_n = 256;
+  else if (d.N > 64) block_n = 128;
   else if (d.N > 32) block_n = 64;
   else if (d.N > 16) block_n = 32;
   else block_n = 16;
@@ -562,20 +605,16 @@ static uav_status_t launch_igemm(const IgemmDesc& d, cudaStream_t stream) {
   p.num_taps = d.num_taps;
   p.k_per_tap = d.k_per_tap;
   p.kblocks_per_tap = (d.k_per_tap + BLOCK_K - 1) / BLOCK_K;
-  uint64_t m_tiles = 1;
   uint32_t box_prod = 1;
   for (int i = 0; i < 5; ++i) {
     p.box[i] = d.box[i];
     p.tiles[i] = d.tiles[i];
     p.out_dims[i] = d.out_dims[i];
-    if (i >= 1) {
-      m_tiles *= d.tiles[i];
-      box_prod *= d.box[i];
-    }
+    if (i >= 1) box_prod *= d.box[i];
   }
   UAV_REQUIRE(box_prod == BLOCK_M && d.box[0] == 64, "igemm: M-tile box must cover 128 rows");
   p.N = (int32_t)d.N;
-  p.n_out = (int32_t)(geglu ? d.N / 2 : d.N);
+  p.n_out = (int32_t)n_out;
   const int out_tile_n = geglu ? block_n / 2 : block_n;
   p.n_tiles = (uint32_t)((p.n_out + out_tile_n - 1) / out_tile_n);
   UAV_REQUIRE(m_tiles * p.n_tiles < (1ull << 31), "igemm: too many tiles");
@@ -646,8 +685,9 @@ static uav_status_t launch_igemm(const IgemmDesc& d, cudaStream_t stream) {
     }
   }
 
-  if (geglu) return launch_instance<128, true>(p, stream);
+  if (geglu) return block_n == 256 ? launch_instance<256, true>(p, stream) : launch_instance<128, true>(p, stream);
   switch (block_n) {
+    case 256: return launch_instance<256, false>(p, stream);
     case 128: return launch_instance<128, false>(p, stream);
     case 64: return launch_instance<64, false>(p, stream);
     case 32: return launch_instance<32, false>(p, stream);
