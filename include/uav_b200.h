@@ -245,10 +245,12 @@ uav_status_t uav_attention(const void* q, const void* k, const void* v, void* ou
                            int64_t ldk, int64_t ldv, int64_t ldo, int64_t kv_batch_div,
                            float scale, uav_stream_t stream);
 
-/* TemporalAttention._attention (attention.py:699-733): per pixel, sequence = frames (F <= 8);
+/* TemporalAttention._attention (attention.py:699-733): per pixel, sequence = frames (any F >= 1);
  * q is scaled, q and k get the rotary embedding on dims [0,32) (cos/sin table rot[F][16][2]),
  * scores += rel_bias[heads][F][F], row-max subtract, softmax, PV.  Tokens are ordered
- * (b, f, hw) — the channels-last video layout — so no rearrange copies are needed. */
+ * (b, f, hw) — the channels-last video layout — so no rearrange copies are needed.  head_dim 64
+ * or 128.  F <= 8 runs on the windowed-pipeline kernels; F > 8 on an online-softmax kernel that
+ * streams 16-frame key tiles. */
 uav_status_t uav_temporal_attention(const void* q, const void* k, const void* v, void* out,
                                     int64_t B, int64_t F, int64_t HW, int heads, int head_dim,
                                     int64_t ldq, int64_t ldk, int64_t ldv, int64_t ldo,
@@ -318,6 +320,13 @@ uav_status_t uav_propagate_step(const void* feat_prop, const void* feat_cur, con
                                 int64_t cs_prop, int64_t cs_cur, int64_t cs_out,
                                 int64_t cs_flow_prop, int64_t cs_flow_check, int nearest, int fuse,
                                 float fuse_scale, float alpha1, float alpha2, int dtype, uav_stream_t stream);
+/* the flow resize of Propagation.forward (propagation_module.py:206-209):
+ * out = F.interpolate(in, (t_out, h_out, w_out), mode='area') * scale, bit-identical to torch's CUDA
+ * kernel (fp32 window sum, one divide, rounded to dtype, then * scale in fp32 and rounded again).
+ * in: [planes][t_in][h_in][w_in], out: [planes][t_out][h_out][w_out], both contiguous. */
+uav_status_t uav_flow_resize_area(const void* in, void* out, int64_t planes, int64_t t_in, int64_t h_in,
+                                  int64_t w_in, int64_t t_out, int64_t h_out, int64_t w_out, float scale,
+                                  int dtype, uav_stream_t stream);
 
 /* ---- after the decode: colour fix + output packing (SURVEY.md §8f rank 4) ---------------------------------
  * All tensors are the reference's planar fp32 "t c h w" frames (planes = t * c). */

@@ -35,6 +35,21 @@ ms = timeit(lambda: ops.temporal_attention(q, k, v, heads, rot, bias, out=out), 
 print(json.dumps({"name": "temporal attn 2x8x46080 h8 d64",
                   "ms": ms, "GBps": 4 * B * Fr * HW * C * 2 / ms / 1e6}))
 
+# clips longer than 8 frames (online-softmax kernel) at the largest temporal-attention site of the h720 UNet:
+# B=2, 90x160 pixels, 8 heads x 64
+for Fr in (16, 32):
+    B, HW, heads, d = 2, 90 * 160, 8, 64
+    C = heads * d
+    qkv = torch.randn(B, Fr, HW, 3 * C, device="cuda").half()
+    q, k, v = qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:]
+    ang = torch.arange(Fr).float()[:, None] * freqs[None, :]
+    rot = torch.stack([ang.cos(), ang.sin()], dim=-1).contiguous().cuda()
+    bias = (torch.randn(heads, Fr, Fr) * 0.3).cuda()
+    out = torch.empty(B, Fr, HW, C, device="cuda", dtype=torch.float16)
+    ms = timeit(lambda: ops.temporal_attention(q, k, v, heads, rot, bias, out=out), iters=10, warmup=3)
+    print(json.dumps({"name": f"temporal attn 2x{Fr}x{HW} h8 d64",
+                      "ms": ms, "GBps": 4 * B * Fr * HW * C * 2 / ms / 1e6}))
+
 # text cross-attention at the top UNet level: 16 frames x 46080 queries, 77 keys, 8 heads x 64 (4 B/element stream of q, o)
 B, heads, d, nq, nk = 16, 8, 64, 46080, 77
 C = heads * d

@@ -86,6 +86,7 @@ _PROTOS = {
     "uav_ddim_step_vt": [P, P, P, P, I64, I32, F32, F32, F32, F32, I32, F32, F32, P, I32, P],
     "uav_add_noise": [P, P, P, I64, F32, F32, I32, P],
     "uav_propagate_step": [P, P, P, P, P, I64, I64, I64, I64, I64, I64, I64, I64, I32, I32, F32, F32, F32, I32, P],
+    "uav_flow_resize_area": [P, P, I64, I64, I64, I64, I64, I64, I64, F32, I32, P],
     "uav_conv2d_taps": [P, I64, I64, I64, I64, I64, P, I64, I32, I32, I32, I32, P, EP, P],
     "uav_instnorm_relu": [P, I64, I64, I64, F32, I32, P, P, P],
     "uav_add_relu": [P, P, P, I64, P],

@@ -7,12 +7,14 @@
 //    spatial self-attention, N = h*w) and d = 512 (VAE mid-block attention, 1 head) run on the
 //    wgmma kernel of attention_tc.cu, and d = 64 on a FlashAttention-2 style mma.sync.m16n8k16
 //    kernel (fp16 in, fp32 accumulate, fp32 online softmax).
-//  * uav_temporal_attention: the seq = T <= 8 per-pixel attention with rotary embedding on
-//    the first 32 dims and the T5-style relative-position bias (attention.py:699-733) as a
-//    register-resident warp kernel: one warp per (pixel, head), lane = (frame, quarter of the
-//    head dim), K/V exchanged with warp shuffles.  Reads q/k/v in the (b, f, hw, c) layout,
-//    so the reference's two "(b f) d c <-> (b d) f c" rearrange copies (attention.py:555,560)
-//    do not exist.
+//  * uav_temporal_attention: the seq = T per-pixel attention with rotary embedding on the
+//    first 32 dims and the T5-style relative-position bias (attention.py:699-733).  T <= 8 (the
+//    pipeline's windows) runs on an mma.sync kernel for a pair of heads, or on a register-resident
+//    warp kernel for an odd head count: one warp per (pixel, head), lane = (frame, quarter of the
+//    head dim), K/V exchanged with warp shuffles.  T > 8 runs on an mma.sync kernel with an
+//    online softmax over 16-frame key tiles.  All read q/k/v in the (b, f, hw, c) layout, so the
+//    reference's two "(b f) d c <-> (b d) f c" rearrange copies (attention.py:555,560) do not
+//    exist.
 #include "uav_common.cuh"
 
 #include <atomic>
@@ -715,6 +717,206 @@ __global__ void __launch_bounds__(128)
   }
 }
 
+// ---------------------------------------------------------------------------------------
+// temporal attention for F > 8 frames (clips longer than the pipeline's 8-frame windows): one warp per
+// (batch, pixel, head).  Queries are taken in 16-frame tiles; keys and values stream through per-warp
+// shared memory in 16-frame tiles and the softmax is online (running fp32 row max and sum, O
+// rescaled), so F has no upper bound.  Rotary is applied in fp32 while the mma fragments of dims
+// [0, 32) are built, as hi + lo fp16 pairs.  Padded key columns are masked to -inf; padded query
+// rows compute on zeros and are never stored.
+// ---------------------------------------------------------------------------------------
+template <int D>
+__global__ void __launch_bounds__(128)
+    temporal_attn_long_kernel(const TaParams p) {
+  constexpr int CH = D / 8;               // 16-byte chunks per row
+  constexpr int LD_ITERS = 16 * CH / 32;  // chunks per lane and tile
+  __shared__ __align__(16) __half smem[4][3][16 * D];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t wid = static_cast<int64_t>(blockIdx.x) * 4 + warp;
+  const int64_t total = static_cast<int64_t>(p.B) * p.HW * p.heads;
+  if (wid >= total) return;  // whole warp
+  const int h = static_cast<int>(wid % p.heads);
+  const int64_t pix = (wid / p.heads) % p.HW;
+  const int64_t b = wid / (static_cast<int64_t>(p.heads) * p.HW);
+  const int64_t F = p.F;
+  __half* sQ = smem[warp][0];
+  __half* sK = smem[warp][1];
+  __half* sV = smem[warp][2];
+  const float* bias_h = p.bias + static_cast<int64_t>(h) * F * F;
+
+  // 16 frames from f0 of one tensor -> swizzled smem tile with cp.async (zero fill past F).  A lane always holds
+  // chunk lane % CH of rows lane / CH + i * (32 / CH).
+  const int chunk = lane % CH;
+  auto load_tile = [&](__half* dst, const __half* src, int64_t ld, int64_t f0) {
+#pragma unroll 1
+    for (int i = 0; i < LD_ITERS; ++i) {
+      const int row = lane / CH + i * (32 / CH);
+      const int64_t frame = f0 + row;
+      const bool ok = frame < F;
+      cp_async16(tile_ptr<D>(dst, row, chunk), src + ((b * F + (ok ? frame : 0)) * p.HW + pix) * ld + h * D + chunk * 8,
+                 ok);
+    }
+  };
+  // rotary on dims [0, 32), computed in fp32 straight into mma fragments and split into hi + lo fp16 parts, so that the
+  // scores see the rotated operands to ~2^-22 instead of one fp16 rounding: pair (x0, x1) of frame f at dims
+  // [dim, dim + 1] -> (x0 c - x1 s, x1 c + x0 s) with (c, s) = rot[f][dim / 2]
+  auto rope_pair = [&](const __half* tile, int row, int dim, int64_t frame, uint32_t& hi, uint32_t& lo) {
+    const float2 x = __half22float2(*reinterpret_cast<const __half2*>(tile_ptr<D>(const_cast<__half*>(tile), row, dim >> 3) +
+                                                                       (dim & 7)));
+    const float2 cs = __ldg(reinterpret_cast<const float2*>(p.rot) + (frame < F ? frame : F - 1) * 16 + (dim >> 1));
+    const float r0 = x.x * cs.x - x.y * cs.y, r1 = x.y * cs.x + x.x * cs.y;
+    const __half2 h = __floats2half2_rn(r0, r1);
+    const float2 hf = __half22float2(h);
+    const __half2 l = __floats2half2_rn(r0 - hf.x, r1 - hf.y);
+    hi = *reinterpret_cast<const uint32_t*>(&h);
+    lo = *reinterpret_cast<const uint32_t*>(&l);
+  };
+
+  const int g = lane >> 2, t4 = lane & 3;
+  const int arow = (lane & 7) + ((lane >> 3) & 1) * 8, achk = lane >> 4;
+  const int brow = (lane & 7) + (lane >> 4) * 8, bchk = (lane >> 3) & 1;
+  const int vrow = (lane & 7) + ((lane >> 3) & 1) * 8;
+#pragma unroll 1
+  for (int64_t q0 = 0; q0 < F; q0 += 16) {
+    __syncwarp();  // the previous tile's output rows have left sQ
+    load_tile(sQ, p.q, p.ldq, q0);
+    cp_async_commit();
+    cp_async_wait<0>();
+    __syncwarp();
+    const int64_t r0 = q0 + g, r1 = q0 + g + 8;  // the two query rows of this lane
+    // A fragments of the rotated dims [0, 32): a[j] = rows g + 8 (j & 1), dims kk*16 + 2 t4 + 8 (j >> 1)
+    uint32_t qh[2][4], ql[2][4];
+#pragma unroll
+    for (int kk = 0; kk < 2; ++kk)
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        rope_pair(sQ, g + (j & 1) * 8, kk * 16 + 2 * t4 + (j >> 1) * 8, j & 1 ? r1 : r0, qh[kk][j], ql[kk][j]);
+    float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+    float o[D / 8][4];
+#pragma unroll
+    for (int i = 0; i < D / 8; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
+
+#pragma unroll 1
+    for (int64_t k0 = 0; k0 < F; k0 += 16) {
+      __syncwarp();  // every lane is done with the previous K/V tile
+      load_tile(sK, p.k, p.ldk, k0);
+      load_tile(sV, p.v, p.ldv, k0);
+      cp_async_commit();
+      cp_async_wait<0>();
+      __syncwarp();
+      // ---- S = Q K^T: s[nb] holds keys k0 + nb*8 + 2*t4 + {0, 1} of rows g ([0..1]) and g + 8 ([2..3]) ----
+      float s[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+      // rotated dims [0, 32): Qh Kh + Qh Kl + Ql Kh; B fragment of n-block nb = key nb*8 + g, dims kk*16 + 2 t4 + {0, 8}
+#pragma unroll
+      for (int kk = 0; kk < 2; ++kk) {
+#pragma unroll
+        for (int nb = 0; nb < 2; ++nb) {
+          uint32_t kh[2], kl[2];
+#pragma unroll
+          for (int j = 0; j < 2; ++j)
+            rope_pair(sK, nb * 8 + g, kk * 16 + 2 * t4 + j * 8, k0 + nb * 8 + g, kh[j], kl[j]);
+          mma16816(s[nb], qh[kk], kh[0], kh[1]);
+          mma16816(s[nb], qh[kk], kl[0], kl[1]);
+          mma16816(s[nb], ql[kk], kh[0], kh[1]);
+        }
+      }
+#pragma unroll
+      for (int kk = 2; kk < D / 16; ++kk) {
+        uint32_t qa[4], bfr[4];
+        ldmatrix_x4(qa, tile_ptr<D>(sQ, arow, kk * 2 + achk));
+        ldmatrix_x4(bfr, tile_ptr<D>(sK, brow, kk * 2 + bchk));
+        mma16816(s[0], qa, bfr[0], bfr[1]);
+        mma16816(s[1], qa, bfr[2], bfr[3]);
+      }
+      float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+      for (int nb = 0; nb < 2; ++nb) {
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          const int64_t col = k0 + nb * 8 + 2 * t4 + j;
+          float x0 = -INFINITY, x1 = -INFINITY;
+          if (col < F) {
+            x0 = s[nb][j] * p.scale + (r0 < F ? __ldg(bias_h + r0 * F + col) : 0.f);
+            x1 = s[nb][2 + j] * p.scale + (r1 < F ? __ldg(bias_h + r1 * F + col) : 0.f);
+          }
+          s[nb][j] = x0;
+          s[nb][2 + j] = x1;
+          mx0 = fmaxf(mx0, x0);
+          mx1 = fmaxf(mx1, x1);
+        }
+      }
+      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
+      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
+      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+      // key column k0 is always valid, so the new maxima are finite; exp(-inf) = 0 covers the first tile
+      const float n0 = fmaxf(m0, mx0), n1 = fmaxf(m1, mx1);
+      const float c0 = __expf(m0 - n0), c1 = __expf(m1 - n1);
+      m0 = n0;
+      m1 = n1;
+      float ps0 = 0.f, ps1 = 0.f;
+#pragma unroll
+      for (int nb = 0; nb < 2; ++nb) {
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          s[nb][j] = __expf(s[nb][j] - n0);
+          s[nb][2 + j] = __expf(s[nb][2 + j] - n1);
+          ps0 += s[nb][j];
+          ps1 += s[nb][2 + j];
+        }
+      }
+      l0 = l0 * c0 + ps0;  // per-lane partial sums: the quad is reduced once at the end
+      l1 = l1 * c1 + ps1;
+#pragma unroll
+      for (int i = 0; i < D / 8; ++i) {
+        o[i][0] *= c0;
+        o[i][1] *= c0;
+        o[i][2] *= c1;
+        o[i][3] *= c1;
+      }
+      // ---- O += P V: the S accumulators are the A fragment of the k = 16 keys step ----
+      uint32_t a[4];
+      {
+        __half2 h0 = __floats2half2_rn(s[0][0], s[0][1]), h1 = __floats2half2_rn(s[0][2], s[0][3]);
+        __half2 h2 = __floats2half2_rn(s[1][0], s[1][1]), h3 = __floats2half2_rn(s[1][2], s[1][3]);
+        a[0] = *reinterpret_cast<uint32_t*>(&h0);
+        a[1] = *reinterpret_cast<uint32_t*>(&h1);
+        a[2] = *reinterpret_cast<uint32_t*>(&h2);
+        a[3] = *reinterpret_cast<uint32_t*>(&h3);
+      }
+#pragma unroll
+      for (int nb = 0; nb < D / 16; ++nb) {
+        uint32_t bfr[4];
+        ldmatrix_x4_trans(bfr, tile_ptr<D>(sV, vrow, nb * 2 + (lane >> 4)));
+        mma16816(o[nb * 2], a, bfr[0], bfr[1]);
+        mma16816(o[nb * 2 + 1], a, bfr[2], bfr[3]);
+      }
+    }
+    l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+    l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+    const float i0 = 1.f / l0, i1 = 1.f / l1;
+    // ---- O -> smem (Q tile) -> 16-byte stores of the rows < F ----
+    __syncwarp();
+#pragma unroll
+    for (int n = 0; n < D / 8; ++n) {
+      *reinterpret_cast<__half2*>(tile_ptr<D>(sQ, g, n) + 2 * t4) = __floats2half2_rn(o[n][0] * i0, o[n][1] * i0);
+      *reinterpret_cast<__half2*>(tile_ptr<D>(sQ, g + 8, n) + 2 * t4) = __floats2half2_rn(o[n][2] * i1, o[n][3] * i1);
+    }
+    __syncwarp();
+#pragma unroll
+    for (int i = 0; i < LD_ITERS; ++i) {
+      const int row = lane / CH + i * (32 / CH);
+      const int64_t frame = q0 + row;
+      if (frame < F) {
+        stg16(p.o + ((b * F + frame) * p.HW + pix) * p.ldo + h * D + chunk * 8,
+              *reinterpret_cast<const uint4*>(tile_ptr<D>(sQ, row, chunk)));
+      }
+    }
+  }
+}
+
 uav_status_t attention_tc(const void* q, const void* k, const void* v, void* out, int64_t batch,
                           int heads, int head_dim, int64_t nq, int64_t nk, int64_t ldq, int64_t ldk,
                           int64_t ldv, int64_t ldo, int64_t kv_batch_div, float scale,
@@ -792,8 +994,8 @@ uav_status_t uav_temporal_attention(const void* q, const void* k, const void* v,
   cudaStream_t stream = (cudaStream_t)stream_;
   UAV_REQUIRE(q && k && v && out && rot_cos_sin && rel_bias,
               "uav_temporal_attention: null pointer");
-  UAV_REQUIRE(B > 0 && F > 0 && F <= 8 && HW > 0 && heads > 0,
-              "uav_temporal_attention: bad shape (F=%lld must be <= 8)", (long long)F);
+  UAV_REQUIRE(B > 0 && F >= 1 && HW > 0 && heads > 0, "uav_temporal_attention: bad shape");
+  UAV_REQUIRE(B <= INT32_MAX && F <= INT32_MAX, "uav_temporal_attention: B or F too large");
   UAV_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0,
               "uav_temporal_attention: token strides must be multiples of 8");
   TaParams p;
@@ -803,7 +1005,17 @@ uav_status_t uav_temporal_attention(const void* q, const void* k, const void* v,
   p.scale = scale; p.rot = rot_cos_sin; p.bias = rel_bias;
   const int64_t warps = B * HW * heads;
   const unsigned grid = (unsigned)((warps + 7) / 8);
-  if (heads % 2 == 0 && (head_dim == 64 || head_dim == 128)) {
+  if (F > 8) {
+    // longer than the pipeline's windows: online softmax over 16-frame key tiles, one warp per (pixel, head)
+    UAV_REQUIRE((warps + 3) / 4 <= INT32_MAX, "uav_temporal_attention: too many (pixel, head) items");
+    const unsigned grid4 = (unsigned)((warps + 3) / 4);
+    if (head_dim == 64) temporal_attn_long_kernel<64><<<grid4, 128, 0, stream>>>(p);
+    else if (head_dim == 128) temporal_attn_long_kernel<128><<<grid4, 128, 0, stream>>>(p);
+    else {
+      set_last_error("uav_temporal_attention: head_dim %d unsupported (64, 128)", head_dim);
+      return UAV_ERR_UNSUPPORTED;
+    }
+  } else if (heads % 2 == 0 && (head_dim == 64 || head_dim == 128)) {
     // mma.sync formulation: one warp per pair of heads
     const unsigned grid2 = (unsigned)((warps / 2 + 3) / 4);
     if (head_dim == 64) temporal_attn_mma_kernel<64><<<grid2, 128, 0, stream>>>(p);

@@ -1,6 +1,7 @@
 // sampler.cu — the per-step elementwise part of VideoUpscalePipeline.__call__
 // (SURVEY.md §8a rows a15, a16, a17): classifier-free-guidance combine, window blend, the
-// split DDIM step (step_v0 / step_vt), add_noise and flow-guided latent propagation.
+// split DDIM step (step_v0 / step_vt), add_noise and flow-guided latent propagation with its
+// area resize of the flows.
 //
 // These run on the reference's own "b c t h w" latents (4 channels).  In fp16 the reference
 // rounds after EVERY torch op (0-dim fp32 scalars x fp16 CUDA tensors -> fp16; SURVEY.md
@@ -233,6 +234,46 @@ __global__ void propagate_step_kernel(const void* feat_prop_, const void* feat_c
   }
 }
 
+// ---------------------------------------------------------------------------------------
+// flow resize of Propagation.forward (propagation_module.py:206-209):
+//   F.interpolate(flows, (t_out, h_out, w_out), mode='area') * scale
+// = adaptive_avg_pool3d: output (ot, oh, ow) averages the input window [floor(i*in/out),
+// ceil((i+1)*in/out)) in each dimension.  As torch's CUDA kernel: fp32 sum in (t, h, w) order,
+// one divide by the window size, rounded to the storage dtype; then `* scale` in fp32 opmath and
+// rounded again.  in/out are (planes, t, h, w) contiguous.
+// ---------------------------------------------------------------------------------------
+__device__ __forceinline__ int64_t area_start(int64_t o, int64_t out_size, int64_t in_size) {
+  return (o * in_size) / out_size;
+}
+__device__ __forceinline__ int64_t area_end(int64_t o, int64_t out_size, int64_t in_size) {
+  return ((o + 1) * in_size + out_size - 1) / out_size;
+}
+
+template <bool HALF>
+__global__ void flow_resize_area_kernel(const void* in_, void* out_, int64_t planes, int64_t t_in,
+                                        int64_t h_in, int64_t w_in, int64_t t_out, int64_t h_out,
+                                        int64_t w_out, float scale) {
+  using N = Num<HALF>;
+  const typename N::T* in = reinterpret_cast<const typename N::T*>(in_);
+  typename N::T* out = reinterpret_cast<typename N::T*>(out_);
+  const int64_t n = planes * t_out * h_out * w_out;
+  UAV_GRID_STRIDE(i, n) {
+    const int64_t ow = i % w_out, oh = (i / w_out) % h_out, ot = (i / (w_out * h_out)) % t_out;
+    const int64_t pl = i / (w_out * h_out * t_out);
+    const int64_t t0 = area_start(ot, t_out, t_in), t1 = area_end(ot, t_out, t_in);
+    const int64_t y0 = area_start(oh, h_out, h_in), y1 = area_end(oh, h_out, h_in);
+    const int64_t x0 = area_start(ow, w_out, w_in), x1 = area_end(ow, w_out, w_in);
+    float sum = 0.f;
+    for (int64_t t = t0; t < t1; ++t) {
+      const int64_t base = (pl * t_in + t) * h_in;
+      for (int64_t y = y0; y < y1; ++y)
+        for (int64_t x = x0; x < x1; ++x) sum = __fadd_rn(sum, N::ld(in, (base + y) * w_in + x));
+    }
+    const float avg = N::rh(__fdiv_rn(sum, static_cast<float>((t1 - t0) * (y1 - y0) * (x1 - x0))));
+    N::st(out, i, N::mul(avg, scale));
+  }
+}
+
 static inline unsigned sgrid(int64_t n) {
   int64_t g = (n + 255) / 256;
   const int64_t cap = static_cast<int64_t>(num_sms()) * 16;
@@ -326,6 +367,17 @@ uav_status_t uav_propagate_step(const void* feat_prop, const void* feat_cur, con
                      flow_prop, flow_check, out, (int)C, (int)H, (int)W, cs_prop, cs_cur, cs_out,
                      cs_flow_prop, cs_flow_check, nearest, fuse, fuse_scale, alpha1, alpha2, inv_wm1,
                      inv_hm1);
+  return UAV_OK;
+}
+
+uav_status_t uav_flow_resize_area(const void* in, void* out, int64_t planes, int64_t t_in, int64_t h_in,
+                                  int64_t w_in, int64_t t_out, int64_t h_out, int64_t w_out, float scale,
+                                  int dtype, uav_stream_t stream) {
+  UAV_REQUIRE(in && out, "uav_flow_resize_area: null pointer");
+  UAV_REQUIRE(planes > 0 && t_in > 0 && h_in > 0 && w_in > 0 && t_out > 0 && h_out > 0 && w_out > 0,
+              "uav_flow_resize_area: bad shape");
+  UAV_DISPATCH_DTYPE(dtype, flow_resize_area_kernel, sgrid(planes * t_out * h_out * w_out), stream, in,
+                     out, planes, t_in, h_in, w_in, t_out, h_out, w_out, scale);
   return UAV_OK;
 }
 

@@ -685,6 +685,19 @@ def propagate_step(feat_prop, feat_cur, flow_prop, flow_check, out, *, nearest: 
     return out
 
 
+def flow_resize_area(flows: torch.Tensor, size, scale: float):
+    """F.interpolate(flows, size, mode='area') * scale, bit-identical to torch on the GPU.  flows: (b, c, t, h, w) fp16/fp32;
+    size: (t_out, h_out, w_out)."""
+    b, c, t, h, w = flows.shape
+    to, ho, wo = (int(s) for s in size)
+    x = flows.contiguous()
+    out = torch.empty(b, c, to, ho, wo, dtype=x.dtype, device=x.device)
+    lib = _lib.load()
+    _lib.check(lib.uav_flow_resize_area(x.data_ptr(), out.data_ptr(), b * c, t, h, w, to, ho, wo, float(scale), _dt(x),
+                                        _stream()), "uav_flow_resize_area")
+    return out
+
+
 # ---------------------------------------------------------------------------------------
 # after the decode: colour fix + output packing (csrc/postprocess.cu) — planar fp32 "t c h w" frames
 # ---------------------------------------------------------------------------------------

@@ -13,7 +13,6 @@ from torch import nn
 
 from . import ops
 from . import _lib
-from ._lib import UavError
 
 
 class Propagation(nn.Module):
@@ -29,16 +28,18 @@ class Propagation(nn.Module):
     @torch.no_grad()
     def forward(self, x, flows_forward, flows_backward, interpolation="bilinear", mode="fuse", fuse_scale=0.5,
                 alpha1=0.01, alpha2=0.5):
-        """x: (b, c, t, h, w); flows: (b, 2, t-1, h, w), same dtype/device as x.  Returns (b, c, t, h, w)."""
+        """x: (b, c, t, h, w); flows: (b, 2, t_f, h_f, w_f) on x's device.  Returns (b, c, t, h, w).
+        Flows of another shape than (t-1, h, w) are area-resized to it and scaled by w / w_f, in their own dtype, as the
+        reference does (propagation_module.py:206-209); at (t-1, h, w) that resize is the identity and is skipped."""
         _lib.require_cuda(x, "Propagation")
         b, c, t, h, w = x.shape
-        if tuple(flows_forward.shape[2:]) != (t - 1, h, w) or tuple(flows_backward.shape[2:]) != (t - 1, h, w):
-            # the reference area-resizes the flows (propagation_module.py:206-209); the pipeline always passes
-            # flows at latent resolution, where that resize is the identity.
-            raise UavError(f"Propagation: flows must already be at latent resolution {(t - 1, h, w)}, "
-                           f"got {tuple(flows_forward.shape[2:])}")
         if interpolation not in ("nearest", "bilinear") or mode not in ("fuse", "copy"):
             raise ValueError(f"unsupported interpolation/mode {interpolation}/{mode}")
+        s = 1.0 * w / flows_forward.shape[-1]  # both flows take the forward flow's width ratio, as in the reference
+        if tuple(flows_forward.shape[2:]) != (t - 1, h, w) or s != 1.0:
+            flows_forward = ops.flow_resize_area(flows_forward, (t - 1, h, w), s)
+        if tuple(flows_backward.shape[2:]) != (t - 1, h, w) or s != 1.0:
+            flows_backward = ops.flow_resize_area(flows_backward, (t - 1, h, w), s)
         x = x.contiguous()
         ff = flows_forward.to(x.dtype).contiguous()
         fb = flows_backward.to(x.dtype).contiguous()

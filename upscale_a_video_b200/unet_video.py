@@ -25,7 +25,6 @@ from torch import nn
 from . import ops
 from ._config import ConfigMixin
 from . import _lib
-from ._lib import UavError
 from .layers import (CrossAttention, CrossAttnDownBlock3D, CrossAttnUpBlock3D, Ctx, DownBlock3D, EmptyTemporalModule3D,
                      InflatedConv3d, PackedModule, ResnetBlock3D, RotaryEmbedding, TemporalModule3D,
                      UNetMidBlock3DCrossAttn, UpBlock3D, _gn, new_cat_slot)
@@ -230,8 +229,6 @@ class UNetVideoModel(PackedModule, ConfigMixin):
         if encoder_hidden_states is None:
             raise ValueError("encoder_hidden_states is required (cross-attention blocks)")
         B, _, T, H, W = sample.shape
-        if T > 8:
-            raise UavError(f"UNetVideoModel.forward: at most 8 frames per call (got {T}); the pipeline windows longer clips")
         dev = sample.device
         c = Ctx(self._packed())
         cfg = self.config
