@@ -92,6 +92,18 @@ def test_c_abi_error_convention(uav_lib):
     assert st == 1 and b"null" in uav_lib.uav_last_error_string()
     st = uav_lib.uav_conv2d(None, 1, 8, 8, 64, 64, None, 64, 5, 1, 0, None, C.byref(e), None)
     assert st == 1 and b"ksize" in uav_lib.uav_last_error_string()
+    # every implicit-GEMM entry point validates its shape before it encodes or launches anything
+    st = uav_lib.uav_conv_temporal(None, 1, 4, 64, 64, 64, None, 64, 2, None, C.byref(e), None)
+    assert st == 1 and b"k must be 1, 3 or 5" in uav_lib.uav_last_error_string()
+    st = uav_lib.uav_conv3d(None, 1, 2, 8, 8, 0, 64, None, 64, None, C.byref(e), None)
+    assert st == 1 and b"uav_conv3d: bad shape" in uav_lib.uav_last_error_string()
+    st = uav_lib.uav_conv2d_taps(None, 1, 8, 8, 64, 64, None, 64, 3, 3, 3, 1, None, C.byref(e), None)
+    assert st == 1 and b"bad padding" in uav_lib.uav_last_error_string()
+    st = uav_lib.uav_conv2d(None, 1, 7, 8, 64, 64, None, 64, 3, 2, 0, None, C.byref(e), None)
+    assert st == 1 and b"stride 2 needs even H" in uav_lib.uav_last_error_string()
+    e_res = _lib.Epilogue(residual=256, ld_res=64, ld_out=64)
+    st = uav_lib.uav_upsample2x_conv3x3(None, 1, 8, 8, 64, 64, None, 64, None, C.byref(e_res), None)
+    assert st == 1 and b"bias-only fp16 epilogue" in uav_lib.uav_last_error_string()
     st = uav_lib.uav_temporal_attention(None, None, None, None, 1, 9, 4, 8, 64, 512, 512, 512, 512, 0.125, None, None, None)
     assert st == 1
     st = uav_lib.uav_ddim_step_v0(None, None, None, 8, 7, 1.0, 0.0, 0, 1.0, 0, None)

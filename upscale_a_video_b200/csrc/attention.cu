@@ -408,12 +408,8 @@ __global__ void __launch_bounds__(FA_THREADS)
 template <int D, int NB16>
 static uav_status_t launch_cross(const FaParams& p, int batch, cudaStream_t stream) {
   constexpr int smem = (2 * NB16 * 16 * D + 2 * FA_BM * D) * 2;
-  static uint64_t configured = 0;  // per-device bit: cudaFuncSetAttribute applies to the current device only
-  const uint64_t dev_bit = 1ull << (current_device() & 63);
-  if (!(configured & dev_bit)) {
-    UAV_CHECK_CUDA(cudaFuncSetAttribute(cross_attn_kernel<D, NB16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    configured |= dev_bit;
-  }
+  const uav_status_t st = opt_in_smem<cross_attn_kernel<D, NB16>>(smem);
+  if (st != UAV_OK) return st;
   const int ntiles = (p.nq + FA_BM - 1) / FA_BM;
   // enough CTAs to fill the GPU ~4x over, each streaming several query tiles past its resident K/V
   int gx = (num_sms() * 8 + batch * p.heads - 1) / (batch * p.heads);
@@ -924,12 +920,8 @@ uav_status_t attention_tc(const void* q, const void* k, const void* v, void* out
 
 static uav_status_t launch_fa(const FaParams& p, int batch, cudaStream_t stream) {
   constexpr int smem = (FA_BM + 4 * FA_BN) * FA_D * 2;
-  static uint64_t configured = 0;  // per-device bit: cudaFuncSetAttribute applies to the current device only
-  const uint64_t dev_bit = 1ull << (current_device() & 63);
-  if (!(configured & dev_bit)) {
-    UAV_CHECK_CUDA(cudaFuncSetAttribute(flash_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    configured |= dev_bit;
-  }
+  const uav_status_t st = opt_in_smem<flash_attn_kernel>(smem);
+  if (st != UAV_OK) return st;
   dim3 grid((p.nq + FA_BM - 1) / FA_BM, batch * p.heads);
   flash_attn_kernel<<<grid, FA_THREADS, smem, stream>>>(p);
   UAV_CHECK_CUDA(cudaGetLastError());

@@ -239,32 +239,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 }
 
 
-static uav_status_t make_map_3d(CUtensorMap* map, const void* base, int64_t cols, int64_t rows,
-                                int64_t batch, int64_t ld, int64_t bs, uint32_t box_rows) {
-  PFN_encodeTiled encode = get_encode_tiled();
-  UAV_REQUIRE(encode != nullptr, "attention_tc: cuTensorMapEncodeTiled entry point unavailable");
-  cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)rows, (cuuint64_t)batch};
-  cuuint64_t strides[2] = {(cuuint64_t)ld * 2, (cuuint64_t)bs * 2};
-  cuuint32_t box[3] = {64, box_rows, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), dims, strides,
-                      box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  UAV_REQUIRE(r == CUDA_SUCCESS, "attention_tc: cuTensorMapEncodeTiled failed with %d", (int)r);
-  return UAV_OK;
-}
-
 template <int DQK, int DVT, int BN>
 static uav_status_t launch_fa_tc(FaTcParams& p, int64_t batch, int dv_splits, cudaStream_t stream) {
   using Cfg = FaTcCfg<DQK, DVT, BN>;
-  static uint64_t configured = 0;  // per-device bit: cudaFuncSetAttribute applies to the current device only
-  const uint64_t dev_bit = 1ull << (current_device() & 63);
-  if (!(configured & dev_bit)) {
-    UAV_CHECK_CUDA(cudaFuncSetAttribute(fa_tc_kernel<DQK, DVT, BN>,
-                                        cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        Cfg::SMEM_BYTES));
-    configured |= dev_bit;
-  }
+  const uav_status_t st = opt_in_smem<fa_tc_kernel<DQK, DVT, BN>>(Cfg::SMEM_BYTES);
+  if (st != UAV_OK) return st;
   dim3 grid((p.nq + TC_BM - 1) / TC_BM, dv_splits, (unsigned)(batch * p.heads));
   fa_tc_kernel<DQK, DVT, BN><<<grid, TC_THREADS, Cfg::SMEM_BYTES, stream>>>(p);
   UAV_CHECK_CUDA(cudaGetLastError());
@@ -286,10 +265,18 @@ uav_status_t attention_tc(const void* q, const void* k, const void* v, void* out
   const int64_t C = (int64_t)heads * head_dim;
   // kv tile rows: 64 for d = 512 (the 64 x 256 fp32 O slice takes 128 registers per thread), else 128
   const uint32_t bn = head_dim == 512 ? 64 : 128;
+  // (batch, rows, C) at token stride ld, loaded in boxes of 64 columns x box_rows tokens of one batch item
+  auto map_3d = [C](CUtensorMap* map, const void* base, int64_t rows, int64_t nbatch, int64_t ld, uint32_t box_rows,
+                    const char* what) {
+    const cuuint64_t dims[3] = {(cuuint64_t)C, (cuuint64_t)rows, (cuuint64_t)nbatch};
+    const cuuint64_t strides[2] = {(cuuint64_t)ld * 2, (cuuint64_t)(rows * ld) * 2};
+    const cuuint32_t box[3] = {64, box_rows, 1};
+    return encode_tensor_map(map, base, 3, dims, strides, box, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, what);
+  };
   uav_status_t st;
-  if ((st = make_map_3d(&p.map_q, q, C, nq, batch, ldq, nq * ldq, TC_BM)) != UAV_OK) return st;
-  if ((st = make_map_3d(&p.map_k, k, C, nk, batch / kv_batch_div, ldk, nk * ldk, bn)) != UAV_OK) return st;
-  if ((st = make_map_3d(&p.map_v, v, C, nk, batch / kv_batch_div, ldv, nk * ldv, bn)) != UAV_OK) return st;
+  if ((st = map_3d(&p.map_q, q, nq, batch, ldq, TC_BM, "attention_tc(Q)")) != UAV_OK) return st;
+  if ((st = map_3d(&p.map_k, k, nk, batch / kv_batch_div, ldk, bn, "attention_tc(K)")) != UAV_OK) return st;
+  if ((st = map_3d(&p.map_v, v, nk, batch / kv_batch_div, ldv, bn, "attention_tc(V)")) != UAV_OK) return st;
   p.out = reinterpret_cast<__half*>(out);
   p.ldo = ldo;
   p.bso = nq * ldo;

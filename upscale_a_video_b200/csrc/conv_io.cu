@@ -295,12 +295,8 @@ static uav_status_t conv_out_launch(const void* x, int64_t B, int64_t T, int64_t
   }
   constexpr int SMEM = 2 * CO_XS_BYTES + CO_NPAD * CO_C * 2 + CO_TH * CO_TW * 5 * 4;
   static_assert(CO_PIX * CO_YS * 4 <= 2 * CO_XS_BYTES, "Y tile must fit in the activation buffers");
-  static uint64_t configured = 0;  // per-device bit: cudaFuncSetAttribute applies to the current device only
-  const uint64_t dev_bit = 1ull << (current_device() & 63);
-  if (!(configured & dev_bit)) {
-    UAV_CHECK_CUDA(cudaFuncSetAttribute(conv_out_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    configured |= dev_bit;
-  }
+  const uav_status_t st = opt_in_smem<conv_out_fused_kernel>(SMEM);
+  if (st != UAV_OK) return st;
   int64_t grid = num_sms();
   if (grid > p.num_tiles) grid = p.num_tiles;
   conv_out_fused_kernel<<<(unsigned)grid, CO_THREADS, SMEM, stream>>>(p);

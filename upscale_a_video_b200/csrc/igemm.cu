@@ -25,6 +25,8 @@
 #include <string.h>
 
 #include <atomic>
+#include <initializer_list>
+#include <iterator>
 #include <mutex>
 
 #include "uav_common.cuh"
@@ -60,7 +62,12 @@ int num_sms() {
   return n[dev];
 }
 
-PFN_encodeTiled get_encode_tiled() {
+// TMA descriptor encode through the driver entry point (no link-time libcuda dependency)
+typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
+                                    const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
+                                    const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+static PFN_encodeTiled get_encode_tiled() {
   static PFN_encodeTiled fn = nullptr;
   static std::once_flag once;
   std::call_once(once, [] {
@@ -72,6 +79,19 @@ PFN_encodeTiled get_encode_tiled() {
       fn = reinterpret_cast<PFN_encodeTiled>(p);
   });
   return fn;
+}
+
+uav_status_t encode_tensor_map(CUtensorMap* map, const void* base, int rank, const cuuint64_t* dims,
+                               const cuuint64_t* strides, const cuuint32_t* box, CUtensorMapL2promotion l2,
+                               const char* what) {
+  PFN_encodeTiled encode = get_encode_tiled();
+  UAV_REQUIRE(encode != nullptr, "%s: cuTensorMapEncodeTiled entry point unavailable", what);
+  const cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+  const CUresult r = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, rank, const_cast<void*>(base), dims, strides, box,
+                            estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, l2,
+                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  UAV_REQUIRE(r == CUDA_SUCCESS, "%s: cuTensorMapEncodeTiled failed with %d", what, (int)r);
+  return UAV_OK;
 }
 
 // ---------------------------------------------------------------------------------------
@@ -467,36 +487,29 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
 // ---------------------------------------------------------------------------------------
 // host: descriptor + launch
 // ---------------------------------------------------------------------------------------
+// Input view and tap table of one launch.  The view has the channels in dim 0 and the pixels in dims 1..4, which the
+// M-tile box (extents multiplying to 128) tiles; the output pixels have the extents out_dims[1..4].
 struct IgemmDesc {
-  const void* a;
-  int rank_a;                // always encoded as rank 5
-  uint64_t a_dims[5];        // dim0 = channels
-  uint64_t a_strides[5];     // elements; a_strides[0] == 1
-  uint32_t box[5];           // box[0] = 64
-  uint32_t tiles[5];
-  uint32_t out_dims[5];
-  int num_taps;
-  int32_t tap_off[MAX_TAPS][5];
-  int k_per_tap;
-  const void* w;
-  int64_t N;
-  void* out;
-  const uav_epilogue_t* epi;
+  const void* a = nullptr;
+  uint64_t a_dims[5] = {};     // dim0 = channels
+  uint64_t a_strides[5] = {};  // elements; a_strides[0] == 1
+  uint32_t box[5] = {};        // box[0] = 64
+  uint32_t tiles[5] = {};
+  uint32_t out_dims[5] = {};
+  int num_taps = 0;
+  int32_t tap_off[MAX_TAPS][5] = {};
+  int k_per_tap = 0;
   // optional strided output view (elements) for dims 1..4; 0 = dense (derived from ld_out / out_dims).
   // Only the TMA-store epilogue understands it (used by the fused nearest-x2 upsample + 3x3 conv).
-  uint64_t out_strides[5];
+  uint64_t out_strides[5] = {};
 };
 
 template <int BLOCK_N, bool GEGLU, bool TMA_EPI, bool AUX>
 static uav_status_t launch_instance2(IgemmParams& p, cudaStream_t stream) {
   using Cfg = IgemmCfg<BLOCK_N, GEGLU>;
-  static uint64_t configured = 0;  // per-device bit: cudaFuncSetAttribute applies to the current device only
-  const uint64_t dev_bit = 1ull << (current_device() & 63);
-  auto kern = igemm_kernel<BLOCK_N, GEGLU, TMA_EPI, AUX>;
-  if (!(configured & dev_bit)) {
-    UAV_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    configured |= dev_bit;
-  }
+  constexpr auto kern = igemm_kernel<BLOCK_N, GEGLU, TMA_EPI, AUX>;
+  const uav_status_t st = opt_in_smem<kern>(Cfg::SMEM_BYTES);
+  if (st != UAV_OK) return st;
   const uint32_t sms = (uint32_t)num_sms();
   kern<<<p.num_tiles < sms ? p.num_tiles : sms, NUM_THREADS, Cfg::SMEM_BYTES, stream>>>(p);
   UAV_CHECK_CUDA(cudaGetLastError());
@@ -534,20 +547,19 @@ static bool wide_tile_pays(uint64_t m_tiles, int64_t n_out, int64_t out_wide) {
   return (double)waves_wide * WIDE_TILE_COST < (double)waves_narrow;
 }
 
-static uav_status_t launch_igemm(const IgemmDesc& d, cudaStream_t stream) {
-  const uav_epilogue_t* e = d.epi;
+// out[pixel][n] = epilogue(sum over the taps of d of A[pixel + tap][c] * w[n][tap][c]) for the N rows of w
+static uav_status_t launch_igemm(const IgemmDesc& d, const void* w, int64_t N, void* out, const uav_epilogue_t* e,
+                                 cudaStream_t stream) {
   UAV_REQUIRE(e != nullptr, "igemm: epilogue descriptor is NULL");
-  UAV_REQUIRE(d.a && d.w && d.out, "igemm: null pointer");
+  UAV_REQUIRE(d.a && w && out, "igemm: null pointer");
   UAV_REQUIRE(d.k_per_tap > 0 && d.k_per_tap % 8 == 0,
               "igemm: input channels (%d) must be a positive multiple of 8", d.k_per_tap);
   UAV_REQUIRE((reinterpret_cast<uintptr_t>(d.a) & 15) == 0 &&
-                  (reinterpret_cast<uintptr_t>(d.w) & 15) == 0,
+                  (reinterpret_cast<uintptr_t>(w) & 15) == 0,
               "igemm: operands must be 16-byte aligned");
   const bool geglu = e->act == UAV_ACT_GEGLU;
-  UAV_REQUIRE(!geglu || (d.N % 128 == 0), "igemm: GEGLU needs N %% 128 == 0 (N=%lld)",
-              (long long)d.N);
-  PFN_encodeTiled encode = get_encode_tiled();
-  UAV_REQUIRE(encode != nullptr, "igemm: cuTensorMapEncodeTiled entry point unavailable");
+  UAV_REQUIRE(!geglu || (N % 128 == 0), "igemm: GEGLU needs N %% 128 == 0 (N=%lld)",
+              (long long)N);
 
   IgemmParams p;
   memset(&p, 0, sizeof(p));
@@ -557,49 +569,35 @@ static uav_status_t launch_igemm(const IgemmDesc& d, cudaStream_t stream) {
   // quantisation; 128-column tiles for the rest of N > 64.  Single-tap GEMMs without GEGLU (Linear, 1x1 conv) keep
   // 128-column tiles: their short main loop does not hide the twice as long epilogue of a 256-column tile (measured: no
   // gain at K = 2048, 10% slower at K = 512).  GEGLU-256 needs N % 256 == 0 so that the value box never reads gate rows.
-  const int64_t n_out = geglu ? d.N / 2 : d.N;
+  const int64_t n_out = geglu ? N / 2 : N;
   int block_n;
-  if (geglu) block_n = (d.N % 256 == 0 && wide_tile_pays(m_tiles, n_out, 128)) ? 256 : 128;
-  else if (d.N >= 256 && d.num_taps > 1 && wide_tile_pays(m_tiles, n_out, 256)) block_n = 256;
-  else if (d.N > 64) block_n = 128;
-  else if (d.N > 32) block_n = 64;
-  else if (d.N > 16) block_n = 32;
+  if (geglu) block_n = (N % 256 == 0 && wide_tile_pays(m_tiles, n_out, 128)) ? 256 : 128;
+  else if (N >= 256 && d.num_taps > 1 && wide_tile_pays(m_tiles, n_out, 256)) block_n = 256;
+  else if (N > 64) block_n = 128;
+  else if (N > 32) block_n = 64;
+  else if (N > 16) block_n = 32;
   else block_n = 16;
 
-  // A map
-  {
-    cuuint64_t dims[5], strides[4];
-    cuuint32_t box[5], estr[5] = {1, 1, 1, 1, 1};
-    for (int i = 0; i < 5; ++i) {
-      dims[i] = d.a_dims[i];
-      box[i] = d.box[i];
-      UAV_REQUIRE(dims[i] >= 1 && box[i] >= 1 && box[i] <= 256, "igemm: bad A dim/box %d", i);
-    }
-    for (int i = 1; i < 5; ++i) {
-      strides[i - 1] = d.a_strides[i] * 2;
-      UAV_REQUIRE(strides[i - 1] % 16 == 0, "igemm: A stride %d not 16-byte aligned", i);
-    }
-    // L2 promotion 256B: a 128-byte k-block fetch also brings the neighbouring 128 bytes of the row into L2, i.e. the
-    // next k-block of the same rows
-    CUresult r = encode(&p.map_a, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, const_cast<void*>(d.a),
-                        dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    UAV_REQUIRE(r == CUDA_SUCCESS, "igemm: cuTensorMapEncodeTiled(A) failed with %d", (int)r);
+  // A map.  L2 promotion 256B: a 128-byte k-block fetch also brings the neighbouring 128 bytes of the row into L2, i.e.
+  // the next k-block of the same rows
+  for (int i = 0; i < 5; ++i)
+    UAV_REQUIRE(d.a_dims[i] >= 1 && d.box[i] >= 1 && d.box[i] <= 256, "igemm: bad A dim/box %d", i);
+  cuuint64_t a_strides[4];
+  for (int i = 1; i < 5; ++i) {
+    a_strides[i - 1] = d.a_strides[i] * 2;
+    UAV_REQUIRE(a_strides[i - 1] % 16 == 0, "igemm: A stride %d not 16-byte aligned", i);
   }
+  uav_status_t st;
+  if ((st = encode_tensor_map(&p.map_a, d.a, 5, d.a_dims, a_strides, d.box, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                              "igemm(A)")) != UAV_OK)
+    return st;
   // B map: [N][K_total] K-major
   const int64_t k_total = (int64_t)d.num_taps * d.k_per_tap;
-  {
-    cuuint64_t dims[2] = {(cuuint64_t)k_total, (cuuint64_t)d.N};
-    cuuint64_t strides[1] = {(cuuint64_t)k_total * 2};
-    cuuint32_t box[2] = {64, (cuuint32_t)(geglu ? block_n / 2 : block_n)};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = encode(&p.map_b, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(d.w), dims,
-                        strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    UAV_REQUIRE(r == CUDA_SUCCESS, "igemm: cuTensorMapEncodeTiled(B) failed with %d", (int)r);
-  }
+  const cuuint64_t b_dims[2] = {(cuuint64_t)k_total, (cuuint64_t)N}, b_stride = (cuuint64_t)k_total * 2;
+  const cuuint32_t b_box[2] = {64, (cuuint32_t)(geglu ? block_n / 2 : block_n)};
+  if ((st = encode_tensor_map(&p.map_b, w, 2, b_dims, &b_stride, b_box, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                              "igemm(B)")) != UAV_OK)
+    return st;
   UAV_REQUIRE(d.num_taps >= 1 && d.num_taps <= MAX_TAPS, "igemm: bad tap count %d", d.num_taps);
   memcpy(p.tap_off, d.tap_off, sizeof(int32_t) * 5 * d.num_taps);
   p.num_taps = d.num_taps;
@@ -613,7 +611,7 @@ static uav_status_t launch_igemm(const IgemmDesc& d, cudaStream_t stream) {
     if (i >= 1) box_prod *= d.box[i];
   }
   UAV_REQUIRE(box_prod == BLOCK_M && d.box[0] == 64, "igemm: M-tile box must cover 128 rows");
-  p.N = (int32_t)d.N;
+  p.N = (int32_t)N;
   p.n_out = (int32_t)n_out;
   const int out_tile_n = geglu ? block_n / 2 : block_n;
   p.n_tiles = (uint32_t)((p.n_out + out_tile_n - 1) / out_tile_n);
@@ -621,7 +619,7 @@ static uav_status_t launch_igemm(const IgemmDesc& d, cudaStream_t stream) {
   p.num_tiles = (uint32_t)(m_tiles * p.n_tiles);
   auto aligned16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
   const bool can_tma = out_tile_n >= 64 && e->out_dtype == UAV_F16 && p.n_out % 8 == 0 && e->ld_out % 8 == 0 &&
-                       aligned16(d.out) &&
+                       aligned16(out) &&
                        (e->residual == nullptr || (e->ld_res % 8 == 0 && aligned16(e->residual))) &&
                        (e->rowvec == nullptr || (e->ld_rowvec % 8 == 0 && aligned16(e->rowvec)));
   p.res_tma = (can_tma && e->residual != nullptr) ? 1 : 0;
@@ -634,7 +632,7 @@ static uav_status_t launch_igemm(const IgemmDesc& d, cudaStream_t stream) {
   p.act = e->act;
   p.out_dtype = e->out_dtype;
   p.ld_out = e->ld_out;
-  p.out = d.out;
+  p.out = out;
   p.out_scale = e->out_scale == 0.0f ? 1.0f : e->out_scale;
   p.gn_partial = reinterpret_cast<float*>(e->gn_partial);
   p.gn_blocks = e->gn_blocks;
@@ -657,32 +655,22 @@ static uav_status_t launch_igemm(const IgemmDesc& d, cudaStream_t stream) {
   UAV_REQUIRE(d.out_strides[1] == 0 || (can_tma && p.residual == nullptr && p.rowvec == nullptr),
               "igemm: a strided output view needs the TMA-store epilogue without residual / row vector");
   if (can_tma) {
-    cuuint64_t dims[5], strides[4];
-    cuuint32_t box[5], estr[5] = {1, 1, 1, 1, 1};
-    dims[0] = (cuuint64_t)p.n_out;
-    box[0] = 64;
-    uint64_t stride_el = (uint64_t)p.ld_out;
+    // output and residual: n_out columns over the output pixels, stored in boxes of 64 columns x the M-tile box
+    cuuint64_t o_dims[5] = {(cuuint64_t)p.n_out}, o_strides[4], r_strides[4];
+    uint64_t o_el = (uint64_t)p.ld_out, r_el = (uint64_t)p.ld_res;
     for (int i = 1; i < 5; ++i) {
-      dims[i] = d.out_dims[i];
-      box[i] = d.box[i];
-      strides[i - 1] = (d.out_strides[i] ? d.out_strides[i] : stride_el) * 2;
-      stride_el *= d.out_dims[i];
+      o_dims[i] = d.out_dims[i];
+      o_strides[i - 1] = (d.out_strides[i] ? d.out_strides[i] : o_el) * 2;
+      r_strides[i - 1] = r_el * 2;
+      o_el *= d.out_dims[i];
+      r_el *= d.out_dims[i];
     }
-    CUresult r = encode(&p.map_out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, d.out, dims, strides, box,
-                        estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                        CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    UAV_REQUIRE(r == CUDA_SUCCESS, "igemm: cuTensorMapEncodeTiled(out) failed with %d", (int)r);
-    if (p.res_tma) {
-      uint64_t rs = (uint64_t)p.ld_res;
-      for (int i = 1; i < 5; ++i) {
-        strides[i - 1] = rs * 2;
-        rs *= d.out_dims[i];
-      }
-      r = encode(&p.map_res, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, const_cast<__half*>(p.residual), dims, strides, box, estr,
-                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      UAV_REQUIRE(r == CUDA_SUCCESS, "igemm: cuTensorMapEncodeTiled(residual) failed with %d", (int)r);
-    }
+    if ((st = encode_tensor_map(&p.map_out, out, 5, o_dims, o_strides, d.box, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                                "igemm(out)")) != UAV_OK)
+      return st;
+    if (p.res_tma && (st = encode_tensor_map(&p.map_res, p.residual, 5, o_dims, r_strides, d.box,
+                                             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "igemm(residual)")) != UAV_OK)
+      return st;
   }
 
   if (geglu) return block_n == 256 ? launch_instance<256, true>(p, stream) : launch_instance<128, true>(p, stream);
@@ -695,18 +683,75 @@ static uav_status_t launch_igemm(const IgemmDesc& d, cudaStream_t stream) {
   }
 }
 
-// choose the (tw, th) rectangle with tw * th == 128 that wastes the fewest rows
-static void pick_tile_2d(int64_t W, int64_t H, uint32_t* tw, uint32_t* th) {
+// The (tw, th) rectangle with tw * th == 128 that wastes the fewest rows of a W x H image: the M-tile box of every launch
+// over images, and the tiling uav_gn_partial_blocks counts statistics blocks over.
+struct TileRect {
+  uint32_t w, h;
+};
+static TileRect pick_tile_2d(int64_t W, int64_t H) {
+  TileRect best_rect{};
   int64_t best = -1;
   for (uint32_t w = 128; w >= 1; w >>= 1) {
     const uint32_t h = 128 / w;
     const int64_t cover = ((W + w - 1) / w) * w * ((H + h - 1) / h) * h;
     if (best < 0 || cover < best) {
       best = cover;
-      *tw = w;
-      *th = h;
+      best_rect = {w, h};
     }
   }
+  return best_rect;
+}
+
+// Dense channels-last input view: `channels` channels at pixel stride `ld`, under the outer extents ext (innermost
+// first), tiled by the M-tile box.  The output pixels have the same extents.
+static void dense_view(IgemmDesc& d, const void* x, int64_t ld, int64_t channels, const int64_t (&ext)[4],
+                       const uint32_t (&box)[4]) {
+  d.a = x;
+  d.k_per_tap = (int)channels;
+  d.a_dims[0] = (uint64_t)channels;
+  d.a_strides[0] = 1;
+  d.box[0] = 64;
+  d.tiles[0] = 1;
+  d.out_dims[0] = 1;
+  uint64_t stride = (uint64_t)ld;
+  for (int i = 1; i < 5; ++i) {
+    d.a_dims[i] = (uint64_t)ext[i - 1];
+    d.a_strides[i] = stride;
+    d.box[i] = box[i - 1];
+    d.tiles[i] = (uint32_t)((ext[i - 1] + box[i - 1] - 1) / box[i - 1]);
+    d.out_dims[i] = (uint32_t)ext[i - 1];
+    stride *= (uint64_t)ext[i - 1];
+  }
+}
+
+// One axis of a tap grid: `extent` taps along view dim `dim`, at offsets start, start + 1, ...
+struct TapAxis {
+  int dim, extent, start;
+};
+// Appends every tap of the grid in the order the weights are packed: the first axis outermost, the last one fastest.
+static void add_tap_grid(IgemmDesc& d, std::initializer_list<TapAxis> axes) {
+  int count = 1;
+  for (const TapAxis& ax : axes) count *= ax.extent;
+  for (int t = 0; t < count; ++t) {
+    int32_t* o = d.tap_off[d.num_taps++];
+    int rest = t;
+    for (auto ax = std::rbegin(axes); ax != std::rend(axes); ++ax) {
+      o[ax->dim] = ax->start + rest % ax->extent;
+      rest /= ax->extent;
+    }
+  }
+}
+
+// stride-1 convolution that keeps the image size: a kh x kw window padded by pad_top rows and pad_left columns, weights
+// (Cout, kh, kw, Cin)
+static uav_status_t conv2d_same(const void* x, int64_t NB, int64_t H, int64_t W, int64_t Cin, int64_t ld_in,
+                                const void* w, int64_t Cout, int kh, int kw, int pad_top, int pad_left, void* out,
+                                const uav_epilogue_t* epi, cudaStream_t stream) {
+  const TileRect t = pick_tile_2d(W, H);
+  IgemmDesc d;
+  dense_view(d, x, ld_in, Cin, {W, H, NB, 1}, {t.w, t.h, 1, 1});
+  add_tap_grid(d, {{2, kh, -pad_top}, {1, kw, -pad_left}});
+  return launch_igemm(d, w, Cout, out, epi, stream);
 }
 
 }  // namespace uav
@@ -717,11 +762,11 @@ extern "C" {
 
 int64_t uav_gn_partial_blocks(int64_t w, int64_t h, int64_t images) {
   if (w <= 0 || h <= 0 || images <= 0) return 0;
-  // one block per 16 rows of a 128-row M-tile (the accumulator rows of one consumer warp)
-  if (h == 1) return ((w + 127) / 128) * images * 8;
-  uint32_t tw, th;
-  pick_tile_2d(w, h, &tw, &th);
-  return ((w + tw - 1) / tw) * ((h + th - 1) / th) * images * 8;
+  // One block per 16 rows of a 128-row M-tile (the accumulator rows of one consumer warp).  This must agree block for
+  // block with the launch whose epilogue writes the statistics, so the M-tiles come from pick_tile_2d as in the launches;
+  // for h == 1 it gives (128, 1), the box of uav_linear and uav_conv_temporal.
+  const TileRect t = pick_tile_2d(w, h);
+  return ((w + t.w - 1) / t.w) * ((h + t.h - 1) / t.h) * images * 8;
 }
 
 const char* uav_version(void) { return "uav_b200 0.3 (sm_90a)"; }
@@ -733,28 +778,9 @@ uav_status_t uav_linear(const void* a, int64_t M, int64_t K, int64_t lda, const 
   UAV_REQUIRE(M >= 0 && K > 0 && N > 0 && lda >= K, "uav_linear: bad shape");
   if (M == 0) return UAV_OK;
   IgemmDesc d;
-  memset(&d, 0, sizeof(d));
-  d.a = a;
-  const uint64_t dims[5] = {(uint64_t)K, (uint64_t)M, 1, 1, 1};
-  const uint64_t strides[5] = {1, (uint64_t)lda, (uint64_t)lda * M, (uint64_t)lda * M,
-                               (uint64_t)lda * M};
-  const uint32_t box[5] = {64, 128, 1, 1, 1};
-  for (int i = 0; i < 5; ++i) {
-    d.a_dims[i] = dims[i];
-    d.a_strides[i] = strides[i];
-    d.box[i] = box[i];
-    d.tiles[i] = 1;
-    d.out_dims[i] = 1;
-  }
-  d.tiles[1] = (uint32_t)((M + 127) / 128);
-  d.out_dims[1] = (uint32_t)M;
-  d.num_taps = 1;
-  d.k_per_tap = (int)K;
-  d.w = w;
-  d.N = N;
-  d.out = out;
-  d.epi = epi;
-  return launch_igemm(d, (cudaStream_t)stream);
+  dense_view(d, a, lda, K, {M, 1, 1, 1}, {128, 1, 1, 1});
+  d.num_taps = 1;  // at offset 0
+  return launch_igemm(d, w, N, out, epi, (cudaStream_t)stream);
 }
 
 uav_status_t uav_conv2d(const void* x, int64_t NB, int64_t H, int64_t W, int64_t Cin,
@@ -769,81 +795,47 @@ uav_status_t uav_conv2d(const void* x, int64_t NB, int64_t H, int64_t W, int64_t
               "uav_conv2d: pad_mode 1 needs a stride-2 3x3 conv");
   // a 1x1 stride-1 convolution is a plain GEMM over the NB*H*W pixels (always-full 128-row tiles)
   if (ksize == 1 && stride == 1) return uav_linear(x, NB * H * W, Cin, ld_in, w, Cout, out, epi, stream);
-  IgemmDesc d;
-  memset(&d, 0, sizeof(d));
-  d.a = x;
-  d.w = w;
-  d.N = Cout;
-  d.out = out;
-  d.epi = epi;
-  d.k_per_tap = (int)Cin;
   const int pad = ksize / 2;
-  if (stride == 1) {
-    uint32_t tw, th;
-    pick_tile_2d(W, H, &tw, &th);
-    const uint64_t dims[5] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)NB, 1};
-    const uint64_t strides[5] = {1, (uint64_t)ld_in, (uint64_t)ld_in * W,
-                                 (uint64_t)ld_in * W * H, (uint64_t)ld_in * W * H * NB};
-    const uint32_t box[5] = {64, tw, th, 1, 1};
-    const uint32_t tiles[5] = {1, (uint32_t)((W + tw - 1) / tw), (uint32_t)((H + th - 1) / th),
-                               (uint32_t)NB, 1};
-    const uint32_t odims[5] = {1, (uint32_t)W, (uint32_t)H, (uint32_t)NB, 1};
-    for (int i = 0; i < 5; ++i) {
-      d.a_dims[i] = dims[i];
-      d.a_strides[i] = strides[i];
-      d.box[i] = box[i];
-      d.tiles[i] = tiles[i];
-      d.out_dims[i] = odims[i];
-    }
-    d.num_taps = ksize * ksize;
-    for (int ky = 0; ky < ksize; ++ky)
-      for (int kx = 0; kx < ksize; ++kx) {
-        int32_t* o = d.tap_off[ky * ksize + kx];
-        o[0] = 0;
-        o[1] = kx - pad;
-        o[2] = ky - pad;
-        o[3] = 0;
-        o[4] = 0;
-      }
-  } else {
-    UAV_REQUIRE(H % 2 == 0 && W % 2 == 0, "uav_conv2d: stride 2 needs even H, W (got %lldx%lld)",
-                (long long)H, (long long)W);
-    UAV_REQUIRE(ld_in == Cin, "uav_conv2d: stride 2 needs a dense input (ld_in == Cin)");
-    const int64_t Wo = W / 2, Ho = H / 2;
-    uint32_t tw, th;
-    pick_tile_2d(Wo, Ho, &tw, &th);
-    // phase view: (2C [px*C + c], W/2, 2 [py], H/2, NB)
-    const uint64_t dims[5] = {(uint64_t)(2 * Cin), (uint64_t)Wo, 2, (uint64_t)Ho, (uint64_t)NB};
-    const uint64_t strides[5] = {1, (uint64_t)(2 * Cin), (uint64_t)(W * Cin),
-                                 (uint64_t)(2 * W * Cin), (uint64_t)(H * W * Cin)};
-    const uint32_t box[5] = {64, tw, 1, th, 1};
-    const uint32_t tiles[5] = {1, (uint32_t)((Wo + tw - 1) / tw), 1,
-                               (uint32_t)((Ho + th - 1) / th), (uint32_t)NB};
-    const uint32_t odims[5] = {1, (uint32_t)Wo, 1, (uint32_t)Ho, (uint32_t)NB};
-    for (int i = 0; i < 5; ++i) {
-      d.a_dims[i] = dims[i];
-      d.a_strides[i] = strides[i];
-      d.box[i] = box[i];
-      d.tiles[i] = tiles[i];
-      d.out_dims[i] = odims[i];
-    }
-    d.num_taps = 9;
-    for (int ky = 0; ky < 3; ++ky)
-      for (int kx = 0; kx < 3; ++kx) {
-        // input coordinate = 2*o + k - pad  (pad = 1 for pad_mode 0, 0 for pad_mode 1)
-        const int iy = ky - (pad_mode == 0 ? 1 : 0);  // in {-1,0,1} or {0,1,2}
-        const int ix = kx - (pad_mode == 0 ? 1 : 0);
-        const int py = ((iy % 2) + 2) % 2, px = ((ix % 2) + 2) % 2;
-        const int oy = (iy - py) / 2, ox = (ix - px) / 2;  // exact
-        int32_t* o = d.tap_off[ky * 3 + kx];
-        o[0] = px * (int)Cin;
-        o[1] = ox;
-        o[2] = py;
-        o[3] = oy;
-        o[4] = 0;
-      }
+  if (stride == 1)
+    return conv2d_same(x, NB, H, W, Cin, ld_in, w, Cout, ksize, ksize, pad, pad, out, epi, (cudaStream_t)stream);
+  UAV_REQUIRE(H % 2 == 0 && W % 2 == 0, "uav_conv2d: stride 2 needs even H, W (got %lldx%lld)",
+              (long long)H, (long long)W);
+  UAV_REQUIRE(ld_in == Cin, "uav_conv2d: stride 2 needs a dense input (ld_in == Cin)");
+  const int64_t Wo = W / 2, Ho = H / 2;
+  const TileRect t = pick_tile_2d(Wo, Ho);
+  IgemmDesc d;
+  d.a = x;
+  d.k_per_tap = (int)Cin;
+  // phase view: (2C [px*C + c], W/2, 2 [py], H/2, NB)
+  const uint64_t dims[5] = {(uint64_t)(2 * Cin), (uint64_t)Wo, 2, (uint64_t)Ho, (uint64_t)NB};
+  const uint64_t strides[5] = {1, (uint64_t)(2 * Cin), (uint64_t)(W * Cin),
+                               (uint64_t)(2 * W * Cin), (uint64_t)(H * W * Cin)};
+  const uint32_t box[5] = {64, t.w, 1, t.h, 1};
+  const uint32_t tiles[5] = {1, (uint32_t)((Wo + t.w - 1) / t.w), 1,
+                             (uint32_t)((Ho + t.h - 1) / t.h), (uint32_t)NB};
+  const uint32_t odims[5] = {1, (uint32_t)Wo, 1, (uint32_t)Ho, (uint32_t)NB};
+  for (int i = 0; i < 5; ++i) {
+    d.a_dims[i] = dims[i];
+    d.a_strides[i] = strides[i];
+    d.box[i] = box[i];
+    d.tiles[i] = tiles[i];
+    d.out_dims[i] = odims[i];
   }
-  return launch_igemm(d, (cudaStream_t)stream);
+  d.num_taps = 9;
+  for (int ky = 0; ky < 3; ++ky)
+    for (int kx = 0; kx < 3; ++kx) {
+      // input coordinate = 2*o + k - pad  (pad = 1 for pad_mode 0, 0 for pad_mode 1)
+      const int iy = ky - (pad_mode == 0 ? 1 : 0);  // in {-1,0,1} or {0,1,2}
+      const int ix = kx - (pad_mode == 0 ? 1 : 0);
+      const int py = ((iy % 2) + 2) % 2, px = ((ix % 2) + 2) % 2;
+      const int oy = (iy - py) / 2, ox = (ix - px) / 2;  // exact
+      int32_t* o = d.tap_off[ky * 3 + kx];
+      o[0] = px * (int)Cin;
+      o[1] = ox;
+      o[2] = py;
+      o[3] = oy;
+    }
+  return launch_igemm(d, w, Cout, out, epi, (cudaStream_t)stream);
 }
 
 uav_status_t uav_conv2d_taps(const void* x, int64_t NB, int64_t H, int64_t W, int64_t Cin, int64_t ld_in,
@@ -853,40 +845,7 @@ uav_status_t uav_conv2d_taps(const void* x, int64_t NB, int64_t H, int64_t W, in
   UAV_REQUIRE(kh >= 1 && kw >= 1 && kh * kw <= MAX_TAPS, "uav_conv2d_taps: at most %d taps (got %d x %d)", MAX_TAPS, kh,
               kw);
   UAV_REQUIRE(pad_top >= 0 && pad_top < kh && pad_left >= 0 && pad_left < kw, "uav_conv2d_taps: bad padding");
-  IgemmDesc d;
-  memset(&d, 0, sizeof(d));
-  d.a = x;
-  d.w = w;
-  d.N = Cout;
-  d.out = out;
-  d.epi = epi;
-  d.k_per_tap = (int)Cin;
-  uint32_t tw, th;
-  pick_tile_2d(W, H, &tw, &th);
-  const uint64_t dims[5] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)NB, 1};
-  const uint64_t strides[5] = {1, (uint64_t)ld_in, (uint64_t)ld_in * W, (uint64_t)ld_in * W * H,
-                               (uint64_t)ld_in * W * H * NB};
-  const uint32_t box[5] = {64, tw, th, 1, 1};
-  const uint32_t tiles[5] = {1, (uint32_t)((W + tw - 1) / tw), (uint32_t)((H + th - 1) / th), (uint32_t)NB, 1};
-  const uint32_t odims[5] = {1, (uint32_t)W, (uint32_t)H, (uint32_t)NB, 1};
-  for (int i = 0; i < 5; ++i) {
-    d.a_dims[i] = dims[i];
-    d.a_strides[i] = strides[i];
-    d.box[i] = box[i];
-    d.tiles[i] = tiles[i];
-    d.out_dims[i] = odims[i];
-  }
-  d.num_taps = kh * kw;
-  for (int ky = 0; ky < kh; ++ky)
-    for (int kx = 0; kx < kw; ++kx) {
-      int32_t* o = d.tap_off[ky * kw + kx];
-      o[0] = 0;
-      o[1] = kx - pad_left;
-      o[2] = ky - pad_top;
-      o[3] = 0;
-      o[4] = 0;
-    }
-  return launch_igemm(d, (cudaStream_t)stream);
+  return conv2d_same(x, NB, H, W, Cin, ld_in, w, Cout, kh, kw, pad_top, pad_left, out, epi, (cudaStream_t)stream);
 }
 
 uav_status_t uav_conv_temporal(const void* x, int64_t B, int64_t T, int64_t HW, int64_t Cin,
@@ -896,36 +855,9 @@ uav_status_t uav_conv_temporal(const void* x, int64_t B, int64_t T, int64_t HW, 
               "uav_conv_temporal: bad shape");
   UAV_REQUIRE(k == 1 || k == 3 || k == 5, "uav_conv_temporal: k must be 1, 3 or 5");
   IgemmDesc d;
-  memset(&d, 0, sizeof(d));
-  d.a = x;
-  d.w = w;
-  d.N = Cout;
-  d.out = out;
-  d.epi = epi;
-  d.k_per_tap = (int)Cin;
-  const uint64_t dims[5] = {(uint64_t)Cin, (uint64_t)HW, (uint64_t)T, (uint64_t)B, 1};
-  const uint64_t strides[5] = {1, (uint64_t)ld_in, (uint64_t)ld_in * HW, (uint64_t)ld_in * HW * T,
-                               (uint64_t)ld_in * HW * T * B};
-  const uint32_t box[5] = {64, 128, 1, 1, 1};
-  const uint32_t tiles[5] = {1, (uint32_t)((HW + 127) / 128), (uint32_t)T, (uint32_t)B, 1};
-  const uint32_t odims[5] = {1, (uint32_t)HW, (uint32_t)T, (uint32_t)B, 1};
-  for (int i = 0; i < 5; ++i) {
-    d.a_dims[i] = dims[i];
-    d.a_strides[i] = strides[i];
-    d.box[i] = box[i];
-    d.tiles[i] = tiles[i];
-    d.out_dims[i] = odims[i];
-  }
-  d.num_taps = k;
-  for (int kt = 0; kt < k; ++kt) {
-    int32_t* o = d.tap_off[kt];
-    o[0] = 0;
-    o[1] = 0;
-    o[2] = kt - k / 2;
-    o[3] = 0;
-    o[4] = 0;
-  }
-  return launch_igemm(d, (cudaStream_t)stream);
+  dense_view(d, x, ld_in, Cin, {HW, T, B, 1}, {128, 1, 1, 1});
+  add_tap_grid(d, {{2, k, -k / 2}});
+  return launch_igemm(d, w, Cout, out, epi, (cudaStream_t)stream);
 }
 
 uav_status_t uav_conv3d(const void* x, int64_t B, int64_t T, int64_t H, int64_t W, int64_t Cin,
@@ -933,42 +865,11 @@ uav_status_t uav_conv3d(const void* x, int64_t B, int64_t T, int64_t H, int64_t 
                         const uav_epilogue_t* epi, uav_stream_t stream) {
   UAV_REQUIRE(B > 0 && T > 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0 && ld_in >= Cin,
               "uav_conv3d: bad shape");
+  const TileRect t = pick_tile_2d(W, H);
   IgemmDesc d;
-  memset(&d, 0, sizeof(d));
-  d.a = x;
-  d.w = w;
-  d.N = Cout;
-  d.out = out;
-  d.epi = epi;
-  d.k_per_tap = (int)Cin;
-  uint32_t tw, th;
-  pick_tile_2d(W, H, &tw, &th);
-  const uint64_t dims[5] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)T, (uint64_t)B};
-  const uint64_t strides[5] = {1, (uint64_t)ld_in, (uint64_t)ld_in * W, (uint64_t)ld_in * W * H,
-                               (uint64_t)ld_in * W * H * T};
-  const uint32_t box[5] = {64, tw, th, 1, 1};
-  const uint32_t tiles[5] = {1, (uint32_t)((W + tw - 1) / tw), (uint32_t)((H + th - 1) / th),
-                             (uint32_t)T, (uint32_t)B};
-  const uint32_t odims[5] = {1, (uint32_t)W, (uint32_t)H, (uint32_t)T, (uint32_t)B};
-  for (int i = 0; i < 5; ++i) {
-    d.a_dims[i] = dims[i];
-    d.a_strides[i] = strides[i];
-    d.box[i] = box[i];
-    d.tiles[i] = tiles[i];
-    d.out_dims[i] = odims[i];
-  }
-  d.num_taps = 27;
-  for (int kt = 0; kt < 3; ++kt)
-    for (int ky = 0; ky < 3; ++ky)
-      for (int kx = 0; kx < 3; ++kx) {
-        int32_t* o = d.tap_off[(kt * 3 + ky) * 3 + kx];
-        o[0] = 0;
-        o[1] = kx - 1;
-        o[2] = ky - 1;
-        o[3] = kt - 1;
-        o[4] = 0;
-      }
-  return launch_igemm(d, (cudaStream_t)stream);
+  dense_view(d, x, ld_in, Cin, {W, H, T, B}, {t.w, t.h, 1, 1});
+  add_tap_grid(d, {{3, 3, -1}, {2, 3, -1}, {1, 3, -1}});
+  return launch_igemm(d, w, Cout, out, epi, (cudaStream_t)stream);
 }
 
 uav_status_t uav_upsample2x_conv3x3(const void* x, int64_t NB, int64_t H, int64_t W, int64_t Cin,
@@ -979,48 +880,21 @@ uav_status_t uav_upsample2x_conv3x3(const void* x, int64_t NB, int64_t H, int64_
   UAV_REQUIRE(epi->residual == nullptr && epi->rowvec == nullptr && epi->out_dtype == UAV_F16 && Cout >= 33,
               "uav_upsample2x_conv3x3: bias-only fp16 epilogue with Cout > 32 required");
   const int64_t ld_out = epi->ld_out;
-  uint32_t tw, th;
-  pick_tile_2d(W, H, &tw, &th);
+  const TileRect t = pick_tile_2d(W, H);
   for (int a = 0; a < 2; ++a)
     for (int b = 0; b < 2; ++b) {
       IgemmDesc d;
-      memset(&d, 0, sizeof(d));
-      d.a = x;
-      d.w = reinterpret_cast<const __half*>(w4) + static_cast<int64_t>(a * 2 + b) * Cout * 4 * Cin;
-      d.N = Cout;
-      d.epi = epi;
-      d.k_per_tap = (int)Cin;
-      const uint64_t dims[5] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)NB, 1};
-      const uint64_t strides[5] = {1, (uint64_t)ld_in, (uint64_t)ld_in * W, (uint64_t)ld_in * W * H,
-                                   (uint64_t)ld_in * W * H * NB};
-      const uint32_t box[5] = {64, tw, th, 1, 1};
-      const uint32_t tiles[5] = {1, (uint32_t)((W + tw - 1) / tw), (uint32_t)((H + th - 1) / th), (uint32_t)NB, 1};
-      const uint32_t odims[5] = {1, (uint32_t)W, (uint32_t)H, (uint32_t)NB, 1};
-      for (int i = 0; i < 5; ++i) {
-        d.a_dims[i] = dims[i];
-        d.a_strides[i] = strides[i];
-        d.box[i] = box[i];
-        d.tiles[i] = tiles[i];
-        d.out_dims[i] = odims[i];
-      }
+      dense_view(d, x, ld_in, Cin, {W, H, NB, 1}, {t.w, t.h, 1, 1});
+      // source taps of the collapsed 2x2 filter: phase 0 reads {-1, 0}, phase 1 reads {0, +1}
+      add_tap_grid(d, {{2, 2, a - 1}, {1, 2, b - 1}});
       // output phase (a, b): pixel (2y + a, 2x + b) of the [NB][2H][2W][ld_out] tensor
-      d.out = reinterpret_cast<__half*>(out) + (static_cast<int64_t>(a) * 2 * W + b) * ld_out;
       d.out_strides[1] = 2 * (uint64_t)ld_out;
       d.out_strides[2] = 2 * 2 * (uint64_t)W * ld_out;
       d.out_strides[3] = 4 * (uint64_t)H * W * ld_out;
       d.out_strides[4] = 4 * (uint64_t)H * W * ld_out * NB;
-      // source taps of the collapsed 2x2 filter: phase 0 reads {-1, 0}, phase 1 reads {0, +1}
-      d.num_taps = 4;
-      for (int ty = 0; ty < 2; ++ty)
-        for (int tx = 0; tx < 2; ++tx) {
-          int32_t* o = d.tap_off[ty * 2 + tx];
-          o[0] = 0;
-          o[1] = (b == 0 ? -1 : 0) + tx;
-          o[2] = (a == 0 ? -1 : 0) + ty;
-          o[3] = 0;
-          o[4] = 0;
-        }
-      uav_status_t st = launch_igemm(d, (cudaStream_t)stream);
+      const __half* w_phase = reinterpret_cast<const __half*>(w4) + static_cast<int64_t>(a * 2 + b) * Cout * 4 * Cin;
+      __half* out_phase = reinterpret_cast<__half*>(out) + (static_cast<int64_t>(a) * 2 * W + b) * ld_out;
+      const uav_status_t st = launch_igemm(d, w_phase, Cout, out_phase, epi, (cudaStream_t)stream);
       if (st != UAV_OK) return st;
     }
   return UAV_OK;

@@ -8,6 +8,8 @@
 #include <cuda.h>
 #include <stdint.h>
 
+#include <atomic>
+
 #include "../../include/uav_b200.h"
 
 namespace uav {
@@ -258,11 +260,27 @@ __device__ __forceinline__ void stg16(void* p, const uint4& v) {
   *reinterpret_cast<uint4*>(p) = v;
 }
 
-// TMA descriptor encode through the driver entry point (no link-time libcuda dependency)
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
-                                    const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                                    const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-PFN_encodeTiled get_encode_tiled();
+// ---------------------------------------------------------------------------------------
+// launch plumbing (host)
+// ---------------------------------------------------------------------------------------
+// Encodes the tensor map of an fp16 tensor of `rank` <= 5 dims (dims and box innermost first, `strides` = the byte
+// strides of dims 1..rank-1) with the 128B swizzle that the wgmma operand tiles and the output staging use, unit element
+// strides and zero fill out of bounds.  `what` names the map in the error message.
+uav_status_t encode_tensor_map(CUtensorMap* map, const void* base, int rank, const cuuint64_t* dims,
+                               const cuuint64_t* strides, const cuuint32_t* box, CUtensorMapL2promotion l2,
+                               const char* what);
+
+// Lets Kernel use `bytes` of dynamic shared memory, with one cudaFuncSetAttribute per device: the attribute applies to
+// the current device only.  Every call for one Kernel passes the same `bytes`.
+template <auto Kernel>
+uav_status_t opt_in_smem(int bytes) {
+  static std::atomic<uint64_t> configured{0};  // bit d: done on device d
+  const uint64_t dev_bit = 1ull << (current_device() & 63);
+  if (!(configured.load(std::memory_order_relaxed) & dev_bit)) {
+    UAV_CHECK_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    configured.fetch_or(dev_bit, std::memory_order_relaxed);
+  }
+  return UAV_OK;
+}
 
 }  // namespace uav

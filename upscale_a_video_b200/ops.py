@@ -166,6 +166,17 @@ def _epi(out: torch.Tensor, bias=None, rowvec=None, rows_per_vec=0, residual=Non
     return e
 
 
+def _igemm(fn: str, args, out: torch.Tensor, e: Epilogue, st: Optional[GnStats], flops, nbytes, tag=""):
+    """launch the implicit-GEMM entry point `fn`(*args, out, e, stream), timed as "igemm"; `st` (the statistics requested
+    from `e`, or None) is attached to `out`"""
+    lib = _lib.load()
+    with _timed("igemm", flops, nbytes, tag):
+        _lib.check(getattr(lib, fn)(*args, out.data_ptr(), C.byref(e), _stream()), fn)
+    if st is not None:
+        out.uav_gn = [st]
+    return out
+
+
 def linear(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, *, out=None,
            residual=None, rowvec=None, rows_per_vec=0, act=ACT_NONE, out_dtype=torch.float16, out_scale=1.0,
            gn_stats=False):
@@ -181,13 +192,8 @@ def linear(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None
     assert out.shape[-1] == n_out and out.numel() // n_out == M
     e = _epi(out, bias, rowvec, rows_per_vec, residual, act, out_scale)
     st = _gn_request(out, n_out, M, 1, 1, a.shape[0] if a.dim() > 2 else 1, e) if gn_stats and act != ACT_GEGLU else None
-    lib = _lib.load()
-    with _timed("igemm", 2.0 * M * N * K, 2.0 * (M * K + N * K + M * n_out), f"linear M{M} K{K} N{N} act{act}"):
-        _lib.check(lib.uav_linear(a.data_ptr(), M, K, _pixel_ld(a) if a.dim() > 1 else K, w.data_ptr(), N,
-                                  out.data_ptr(), C.byref(e), _stream()), "uav_linear")
-    if st is not None:
-        out.uav_gn = [st]
-    return out
+    return _igemm("uav_linear", (a.data_ptr(), M, K, _pixel_ld(a) if a.dim() > 1 else K, w.data_ptr(), N), out, e, st,
+                  2.0 * M * N * K, 2.0 * (M * K + N * K + M * n_out), f"linear M{M} K{K} N{N} act{act}")
 
 
 def conv2d(x: torch.Tensor, w: torch.Tensor, bias=None, *, stride=1, pad_mode=0, out=None, residual=None,
@@ -209,15 +215,10 @@ def conv2d(x: torch.Tensor, w: torch.Tensor, bias=None, *, stride=1, pad_mode=0,
     if gn_stats:
         st = (_gn_request(out, Cout, NB * Ho * Wo, 1, 1, lead[0] if lead else 1, e) if (k == 1 and stride == 1) else
               _gn_request(out, Cout, Wo, Ho, NB, lead[0] if lead else 1, e))
-    lib = _lib.load()
-    with _timed("igemm", 2.0 * NB * Ho * Wo * Cout * Cin * k * k,
-                2.0 * (NB * H * W * Cin + w.numel()) + out.element_size() * NB * Ho * Wo * Cout,
-                f"conv{k}x{k}s{stride} {NB}x{H}x{W} {Cin}->{Cout}"):
-        _lib.check(lib.uav_conv2d(x.data_ptr(), NB, H, W, Cin, _pixel_ld(x), w.data_ptr(), Cout, k, stride,
-                                  pad_mode, out.data_ptr(), C.byref(e), _stream()), "uav_conv2d")
-    if st is not None:
-        out.uav_gn = [st]
-    return out
+    return _igemm("uav_conv2d", (x.data_ptr(), NB, H, W, Cin, _pixel_ld(x), w.data_ptr(), Cout, k, stride, pad_mode), out,
+                  e, st, 2.0 * NB * Ho * Wo * Cout * Cin * k * k,
+                  2.0 * (NB * H * W * Cin + w.numel()) + out.element_size() * NB * Ho * Wo * Cout,
+                  f"conv{k}x{k}s{stride} {NB}x{H}x{W} {Cin}->{Cout}")
 
 
 def upsample2x_conv3x3(x: torch.Tensor, w4: torch.Tensor, bias=None, out=None):
@@ -234,12 +235,9 @@ def upsample2x_conv3x3(x: torch.Tensor, w4: torch.Tensor, bias=None, out=None):
         out = torch.empty(*lead, 2 * H, 2 * W, Cout, dtype=torch.float16, device=x.device)
     assert tuple(out.shape) == (*lead, 2 * H, 2 * W, Cout) and out.dtype == torch.float16
     e = _epi(out, bias)
-    lib = _lib.load()
-    with _timed("igemm", 2.0 * NB * 4 * H * W * Cout * Cin * 4, 2.0 * (NB * H * W * Cin + w4.numel() + out.numel()),
-                f"up2x+conv {NB}x{H}x{W} {Cin}->{Cout}"):
-        _lib.check(lib.uav_upsample2x_conv3x3(x.data_ptr(), NB, H, W, Cin, _pixel_ld(x), w4.data_ptr(), Cout,
-                                              out.data_ptr(), C.byref(e), _stream()), "uav_upsample2x_conv3x3")
-    return out
+    return _igemm("uav_upsample2x_conv3x3", (x.data_ptr(), NB, H, W, Cin, _pixel_ld(x), w4.data_ptr(), Cout), out, e,
+                  None, 2.0 * NB * 4 * H * W * Cout * Cin * 4,
+                  2.0 * (NB * H * W * Cin + w4.numel() + out.numel()), f"up2x+conv {NB}x{H}x{W} {Cin}->{Cout}")
 
 
 def collapse_upsample_filter(w: torch.Tensor) -> torch.Tensor:
@@ -268,14 +266,9 @@ def conv_temporal(x: torch.Tensor, w: torch.Tensor, bias=None, *, out=None, resi
         out = torch.empty(B, T, H, W, Cout, dtype=out_dtype, device=x.device)
     e = _epi(out, bias, rowvec, rows_per_vec, residual, act, out_scale)
     st = _gn_request(out, Cout, H * W, 1, B * T, B, e) if gn_stats else None
-    lib = _lib.load()
-    with _timed("igemm", 2.0 * B * T * H * W * Cout * Cin * k, 2.0 * (x.numel() + w.numel() + B * T * H * W * Cout),
-                f"conv_t{k} {B}x{T}x{H}x{W} {Cin}->{Cout}"):
-        _lib.check(lib.uav_conv_temporal(x.data_ptr(), B, T, H * W, Cin, _pixel_ld(x), w.data_ptr(), Cout, k,
-                                         out.data_ptr(), C.byref(e), _stream()), "uav_conv_temporal")
-    if st is not None:
-        out.uav_gn = [st]
-    return out
+    return _igemm("uav_conv_temporal", (x.data_ptr(), B, T, H * W, Cin, _pixel_ld(x), w.data_ptr(), Cout, k), out, e, st,
+                  2.0 * B * T * H * W * Cout * Cin * k, 2.0 * (x.numel() + w.numel() + B * T * H * W * Cout),
+                  f"conv_t{k} {B}x{T}x{H}x{W} {Cin}->{Cout}")
 
 
 def conv3d(x: torch.Tensor, w: torch.Tensor, bias=None, *, out=None, residual=None, act=ACT_NONE,
@@ -289,13 +282,8 @@ def conv3d(x: torch.Tensor, w: torch.Tensor, bias=None, *, out=None, residual=No
         out = torch.empty(B, T, H, W, Cout, dtype=out_dtype, device=x.device)
     e = _epi(out, bias, None, 0, residual, act, out_scale)
     st = _gn_request(out, Cout, W, H, B * T, B, e) if gn_stats else None
-    lib = _lib.load()
-    with _timed("igemm", 2.0 * B * T * H * W * Cout * Cin * 27, 2.0 * (x.numel() + w.numel() + B * T * H * W * Cout)):
-        _lib.check(lib.uav_conv3d(x.data_ptr(), B, T, H, W, Cin, _pixel_ld(x), w.data_ptr(), Cout,
-                                  out.data_ptr(), C.byref(e), _stream()), "uav_conv3d")
-    if st is not None:
-        out.uav_gn = [st]
-    return out
+    return _igemm("uav_conv3d", (x.data_ptr(), B, T, H, W, Cin, _pixel_ld(x), w.data_ptr(), Cout), out, e, st,
+                  2.0 * B * T * H * W * Cout * Cin * 27, 2.0 * (x.numel() + w.numel() + B * T * H * W * Cout))
 
 
 # ------------------------------------------------------------------------------------------------
@@ -779,13 +767,10 @@ def conv2d_taps(x: torch.Tensor, w: torch.Tensor, bias=None, *, pad_top: int, pa
         out = torch.empty(NB, H, W, Cout, dtype=out_dtype, device=x.device)
     assert tuple(out.shape) == (NB, H, W, Cout)
     e = _epi(out, bias, None, 0, residual, act)
-    lib = _lib.load()
-    with _timed("igemm", 2.0 * NB * H * W * Cout * Cin * kh * kw,
-                2.0 * (NB * H * W * Cin + w.numel()) + out.element_size() * NB * H * W * Cout,
-                f"conv{kh}x{kw}taps {NB}x{H}x{W} {Cin}->{Cout}"):
-        _lib.check(lib.uav_conv2d_taps(x.data_ptr(), NB, H, W, Cin, _pixel_ld(x), w.data_ptr(), Cout, kh, kw, pad_top,
-                                       pad_left, out.data_ptr(), C.byref(e), _stream()), "uav_conv2d_taps")
-    return out
+    return _igemm("uav_conv2d_taps", (x.data_ptr(), NB, H, W, Cin, _pixel_ld(x), w.data_ptr(), Cout, kh, kw, pad_top,
+                                      pad_left), out, e, None, 2.0 * NB * H * W * Cout * Cin * kh * kw,
+                  2.0 * (NB * H * W * Cin + w.numel()) + out.element_size() * NB * H * W * Cout,
+                  f"conv{kh}x{kw}taps {NB}x{H}x{W} {Cin}->{Cout}")
 
 
 def instnorm_relu(x: torch.Tensor, relu: bool = True, eps: float = 1e-5) -> torch.Tensor:
