@@ -145,7 +145,8 @@ uav_status_t uav_upsample2x_conv3x3(const void* x, int64_t NB, int64_t H, int64_
 /* ---------------------------------------------------------------------------------------------
  * normalisation
  * ------------------------------------------------------------------------------------------- */
-/* bytes of caller-owned scratch needed by uav_groupnorm_silu (fp64 {sum, sumsq} per (n, group)) */
+/* bytes of caller-owned scratch (`workspace`) needed by uav_groupnorm_silu, uav_groupnorm_silu_from_partials and
+ * uav_groupnorm_affine: fp64 {sum, sumsq} per (n, group) and split, plus the read pass's per-block partials */
 size_t uav_groupnorm_workspace_bytes(int64_t n_outer, int groups);
 
 /* GroupNorm (+ optional SiLU) over channels-last data: x [n_outer][pixels][ld_in] fp16, statistics

@@ -113,6 +113,43 @@ def test_c_abi_error_convention(uav_lib):
     assert uav_lib.uav_launch_count() == 0
 
 
+def test_groupnorm_validates_before_launch(uav_lib):
+    """every GroupNorm entry point runs all its checks before its first launch: a bad call returns status 1 with its
+    message and launches nothing, also when the bad argument is only needed by a later stage (the apply of an unaligned
+    tensor, the tensor of a later source).  The pointers are never dereferenced."""
+    from upscale_a_video_b200 import _lib
+
+    def sources(*specs):  # (C, ld) per source, each with its own fp16 tensor
+        srcs = (_lib.GnSource * len(specs))()
+        for s, (c, ld) in zip(srcs, specs):
+            s.partial, s.blocks, s.C, s.slabs, s.x, s.ld, s.slab_stride = 256, 512, c, 1, 4096, ld, 0
+        return srcs
+
+    def silu(x, C, groups, ws_bytes=None):
+        ws = uav_lib.uav_groupnorm_workspace_bytes(1, groups) if ws_bytes is None else ws_bytes
+        return uav_lib.uav_groupnorm_silu(x, 1, 16, C, C, groups, 256, 256, 1e-5, 1, 256, C, 256, ws, None)
+
+    def from_partials(C, groups, srcs):
+        return uav_lib.uav_groupnorm_silu_from_partials(None, 1, 16, C, C, groups, 256, 256, 1e-5, 1, 256, C, srcs,
+                                                        len(srcs), 256, uav_lib.uav_groupnorm_workspace_bytes(1, groups),
+                                                        None)
+
+    def rejects(st, msg):
+        assert st == 1 and msg in uav_lib.uav_last_error_string(), (st, msg, uav_lib.uav_last_error_string())
+
+    rejects(silu(2, 64, 32), b"uav_groupnorm_silu: C % 8 == 0 tensors must be 16-byte aligned")
+    rejects(from_partials(128, 8, sources((64, 64), (64, 32))), b"uav_groupnorm_silu_from_partials: bad tensor of source 1")
+    rejects(silu(256, 4096, 32), b"uav_groupnorm_silu: C > 2048 unsupported")
+    rejects(silu(256, 64, 32, ws_bytes=16), b"uav_groupnorm_silu: workspace too small")
+    rejects(from_partials(64, 32, sources((64, 64))), b"channels per group (2) must be a multiple of 8")
+    rejects(from_partials(64, 8, sources((60, 64))), b"groupnorm from partials: bad source 0")
+    rejects(from_partials(128, 8, sources((64, 64))), b"sources cover 64 channels, x has 128")
+    rejects(uav_lib.uav_groupnorm_affine(2, 1, 16, 64, 64, 8, 256, 256, 1e-5, None, 0, 256, 256,
+                                         uav_lib.uav_groupnorm_workspace_bytes(1, 8), None),
+            b"uav_groupnorm_affine: without sources x must be an aligned fp16 tensor")
+    assert uav_lib.uav_launch_count() == 0
+
+
 def test_scheduler_host_tables_match_oracle():
     """DDIMScheduler's host-side schedule (timesteps, alphas) is plain CPU math: compare with the oracle without a GPU"""
     import json

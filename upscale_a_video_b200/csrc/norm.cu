@@ -150,87 +150,54 @@ __global__ void __launch_bounds__(256)
 // ---------------------------------------------------------------------------------------
 // apply: y = (x - mean) * rstd * gamma + beta, optional SiLU; fp16 out
 // ---------------------------------------------------------------------------------------
+// {scale, shift} = {gamma[c] * rstd, beta[c] - mean * gamma[c] * rstd} of channel c in group g of slab n, from the
+// fp64 {sum, sumsq} of (n, g) given as `nsplit` partials (added in a fixed order) over cnt elements.  gamma / beta are
+// read after the fp64 math on purpose: passed as values, their loads are hoisted and the kernels' code changes.
+__device__ __forceinline__ float2 gn_scale_shift(const double* __restrict__ sums, int nsplit, int n, int G, int g,
+                                                 double cnt, const float* __restrict__ gamma,
+                                                 const float* __restrict__ beta, int c, float eps) {
+  double s = 0.0, q = 0.0;
+  for (int k = 0; k < nsplit; ++k) {
+    s += sums[((static_cast<int64_t>(n) * G + g) * nsplit + k) * 2];
+    q += sums[((static_cast<int64_t>(n) * G + g) * nsplit + k) * 2 + 1];
+  }
+  const double mean = s / cnt;
+  double var = q / cnt - mean * mean;
+  if (var < 0.0) var = 0.0;
+  const float rstd = static_cast<float>(1.0 / sqrt(var + static_cast<double>(eps)));
+  const float sc = gamma[c] * rstd;
+  return make_float2(sc, beta[c] - static_cast<float>(mean) * sc);
+}
+
+// scalar apply for C % 8 != 0 (the C = 3 GroupNorm of the video VAE's condition input); statistics with nsplit = 1
 __global__ void __launch_bounds__(GN_THREADS)
     gn_apply_kernel(const __half* __restrict__ x, int64_t pixels, int C, int64_t ld_in, int G,
                     const double* __restrict__ sums, const float* __restrict__ gamma,
                     const float* __restrict__ beta, float eps, int silu, __half* __restrict__ y,
                     int64_t ld_out) {
-  extern __shared__ float s_aff[];  // [C] scale, [C] shift
-  float* s_scale = s_aff;
-  float* s_shift = s_aff + C;
+  extern __shared__ float2 s_aff[];  // [C] {scale, shift}
   const int n = blockIdx.y;
   const int cpg = C / G;
   const double cnt = static_cast<double>(pixels) * cpg;
-  for (int c = threadIdx.x; c < C; c += GN_THREADS) {
-    const int g = c / cpg;
-    const double s = sums[(static_cast<int64_t>(n) * G + g) * 2];
-    const double q = sums[(static_cast<int64_t>(n) * G + g) * 2 + 1];
-    const double mean = s / cnt;
-    double var = q / cnt - mean * mean;
-    if (var < 0.0) var = 0.0;
-    const float rstd = static_cast<float>(1.0 / sqrt(var + static_cast<double>(eps)));
-    const float sc = gamma[c] * rstd;
-    s_scale[c] = sc;
-    s_shift[c] = beta[c] - static_cast<float>(mean) * sc;
-  }
+  for (int c = threadIdx.x; c < C; c += GN_THREADS)
+    s_aff[c] = gn_scale_shift(sums, 1, n, G, c / cpg, cnt, gamma, beta, c, eps);
   __syncthreads();
   const __half* xn = x + static_cast<int64_t>(n) * pixels * ld_in;
   __half* yn = y + static_cast<int64_t>(n) * pixels * ld_out;
-  if ((C & 7) == 0) {
-    const int octs = C >> 3;
-    const int64_t total = pixels * octs;
-    const int64_t gstride = static_cast<int64_t>(gridDim.x) * GN_THREADS;
-    auto one = [&](int64_t i, const uint4& v) {
-      const int64_t p = i / octs;
-      const int oct = static_cast<int>(i - p * octs);
-      const __half2* h = reinterpret_cast<const __half2*>(&v);
-      uint4 o;
-      uint32_t* ow = reinterpret_cast<uint32_t*>(&o);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 f = __half22float2(h[j]);
-        const int c = oct * 8 + 2 * j;
-        float a = f.x * s_scale[c] + s_shift[c];
-        float b = f.y * s_scale[c + 1] + s_shift[c + 1];
-        if (silu) {
-          a = silu_f(a);
-          b = silu_f(b);
-        }
-        __half2 r = __floats2half2_rn(a, b);
-        ow[j] = *reinterpret_cast<uint32_t*>(&r);
-      }
-      stg16(yn + p * ld_out + oct * 8, o);
-    };
-    auto src = [&](int64_t i) {
-      const int64_t p = i / octs;
-      return xn + p * ld_in + (i - p * octs) * 8;
-    };
-    int64_t i = static_cast<int64_t>(blockIdx.x) * GN_THREADS + threadIdx.x;
-    for (; i + 3 * gstride < total; i += 4 * gstride) {  // 4 loads in flight per thread
-      const uint4 v0 = ldg16(src(i)), v1 = ldg16(src(i + gstride));
-      const uint4 v2 = ldg16(src(i + 2 * gstride)), v3 = ldg16(src(i + 3 * gstride));
-      one(i, v0);
-      one(i + gstride, v1);
-      one(i + 2 * gstride, v2);
-      one(i + 3 * gstride, v3);
-    }
-    for (; i < total; i += gstride) one(i, ldg16(src(i)));
-  } else {
-    const int64_t total = pixels * C;
-    for (int64_t i = static_cast<int64_t>(blockIdx.x) * GN_THREADS + threadIdx.x; i < total;
-         i += static_cast<int64_t>(gridDim.x) * GN_THREADS) {
-      const int64_t p = i / C;
-      const int c = static_cast<int>(i - p * C);
-      float a = __half2float(xn[p * ld_in + c]) * s_scale[c] + s_shift[c];
-      if (silu) a = silu_f(a);
-      yn[p * ld_out + c] = __float2half_rn(a);
-    }
+  const int64_t total = pixels * C;
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * GN_THREADS + threadIdx.x; i < total;
+       i += static_cast<int64_t>(gridDim.x) * GN_THREADS) {
+    const int64_t p = i / C;
+    const int c = static_cast<int>(i - p * C);
+    float a = __half2float(xn[p * ld_in + c]) * s_aff[c].x + s_aff[c].y;
+    if (silu) a = silu_f(a);
+    yn[p * ld_out + c] = __float2half_rn(a);
   }
 }
 
 // vector path of the apply pass: thread = (pixel lane, 8-channel octet) like the stats kernel, so the 8 scale
 // and 8 shift values of its channels live in registers for the whole pixel loop — no shared-memory
-// lookups per element (the smem version above saturates the LSU pipe at ~3 TB/s).
+// lookups per element (a shared-memory table read per element saturates the LSU pipe at ~3 TB/s).
 __global__ void __launch_bounds__(GN_THREADS)
     gn_apply_vec_kernel(const __half* __restrict__ x, int64_t pixels, int C, int64_t ld_in, int G,
                         const double* __restrict__ sums, int nsplit, const float* __restrict__ gamma,
@@ -251,18 +218,9 @@ __global__ void __launch_bounds__(GN_THREADS)
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
     const int c = chan_off + oct * 8 + j;
-    const int g = c / cpg;
-    double s = 0.0, q = 0.0;
-    for (int k = 0; k < nsplit; ++k) {  // fixed order: the statistics may arrive as `nsplit` partial sums per group
-      s += sums[((static_cast<int64_t>(n) * G + g) * nsplit + k) * 2];
-      q += sums[((static_cast<int64_t>(n) * G + g) * nsplit + k) * 2 + 1];
-    }
-    const double mean = s / cnt;
-    double var = q / cnt - mean * mean;
-    if (var < 0.0) var = 0.0;
-    const float rstd = static_cast<float>(1.0 / sqrt(var + static_cast<double>(eps)));
-    sc[j] = gamma[c] * rstd;
-    sh[j] = beta[c] - static_cast<float>(mean) * sc[j];
+    const float2 a = gn_scale_shift(sums, nsplit, n, G, c / cpg, cnt, gamma, beta, c, eps);
+    sc[j] = a.x;
+    sh[j] = a.y;
   }
   const __half* xn = x + static_cast<int64_t>(n) * x_slab_stride + oct * 8;
   __half* yn = y + static_cast<int64_t>(n) * pixels * ld_out + chan_off + oct * 8;
@@ -358,18 +316,7 @@ __global__ void gn_affine_kernel(const double* __restrict__ sums, int nsplit, in
   const int n = blockIdx.y;
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
-  const int g = c / (C / G);
-  double s = 0.0, q = 0.0;
-  for (int k = 0; k < nsplit; ++k) {
-    s += sums[((static_cast<int64_t>(n) * G + g) * nsplit + k) * 2];
-    q += sums[((static_cast<int64_t>(n) * G + g) * nsplit + k) * 2 + 1];
-  }
-  const double mean = s / cnt;
-  double var = q / cnt - mean * mean;
-  if (var < 0.0) var = 0.0;
-  const float rstd = static_cast<float>(1.0 / sqrt(var + static_cast<double>(eps)));
-  const float sc = gamma[c] * rstd;
-  affine[static_cast<int64_t>(n) * C + c] = make_float2(sc, beta[c] - static_cast<float>(mean) * sc);
+  affine[static_cast<int64_t>(n) * C + c] = gn_scale_shift(sums, nsplit, n, G, c / (C / G), cnt, gamma, beta, c, eps);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -480,6 +427,108 @@ size_t uav_groupnorm_workspace_bytes(int64_t n_outer, int groups) {
   return static_cast<size_t>(n_outer) * groups * (2 * sizeof(double) + GN_MAX_BLOCKS_PER_N * sizeof(float2));
 }
 
+// follows every GroupNorm launch: a launch error is returned, a launch that went in is counted
+#define GN_LAUNCHED()                                   \
+  do {                                                  \
+    UAV_CHECK_CUDA(cudaGetLastError());                 \
+    g_launches.fetch_add(1, std::memory_order_relaxed); \
+  } while (0)
+
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+// gridDim.x of a grid-stride pass over `items` per slab: about `per_sm` CTAs per SM over all n_outer slabs, at most one
+// per `per_block` items, at least one
+static int64_t gn_blocks(int per_sm, int64_t n_outer, int64_t items, int64_t per_block) {
+  const int64_t want = ((int64_t)num_sms() * per_sm + n_outer - 1) / n_outer;
+  const int64_t most = (items + per_block - 1) / per_block;
+  const int64_t b = want < most ? want : most;
+  return b < 1 ? 1 : b;
+}
+
+// statistics stage, read pass over x: per-block partials (the vector kernel when x allows 16-byte loads of whole 4-channel
+// units of a group, else the generic one), then their fp64 reduction -> sums[n][g][S = 1][2] at the head of `workspace`
+static uav_status_t gn_stats_pass(const void* x, int64_t n_outer, int64_t pixels, int64_t C, int64_t ld_in, int groups,
+                                  void* workspace, cudaStream_t stream) {
+  double* sums = reinterpret_cast<double*>(workspace);
+  float2* partial = reinterpret_cast<float2*>(sums + n_outer * groups * 2);
+  const __half* xh = reinterpret_cast<const __half*>(x);
+  const bool vec = (C % 8 == 0) && ((C / groups) % 4 == 0) && (ld_in % 8 == 0) && aligned16(x);
+  // vector kernel: >= ~16 pixels per thread to amortise the block reduction
+  int64_t gx = vec ? gn_blocks(8, n_outer, pixels, GN_THREADS / (C / 8) * 16) : gn_blocks(4, n_outer, pixels, GN_THREADS);
+  if (gx > GN_MAX_BLOCKS_PER_N) gx = GN_MAX_BLOCKS_PER_N;
+  const dim3 grid((unsigned)gx, (unsigned)n_outer);
+  if (vec)
+    gn_stats_kernel<<<grid, GN_THREADS, 0, stream>>>(xh, pixels, (int)C, ld_in, groups, partial);
+  else
+    gn_stats_generic_kernel<<<grid, GN_THREADS, 0, stream>>>(xh, pixels, (int)C, ld_in, groups, partial);
+  GN_LAUNCHED();
+  gn_finalize_kernel<<<dim3((unsigned)groups, (unsigned)n_outer), 256, 0, stream>>>(partial, (int)gx, groups, sums);
+  GN_LAUNCHED();
+  return UAV_OK;
+}
+
+// statistics stage from the producers' blocks, checks: the sources of a C-channel GroupNorm -> `prm` and the split count
+// *S.  Launches nothing, so that a caller can finish its own checks before gn_reduce_sources.
+static uav_status_t gn_reduce_plan(int64_t n_outer, int64_t C, int groups, const uav_gn_source_t* sources, int n_sources,
+                                   size_t workspace_bytes, GnReduceParams* prm, int* S_out) {
+  const int cpg = (int)(C / groups);
+  UAV_REQUIRE(cpg % 8 == 0, "groupnorm from partials: channels per group (%d) must be a multiple of 8", cpg);
+  UAV_REQUIRE(n_sources >= 1 && n_sources <= 4, "groupnorm from partials: 1..4 sources");
+  UAV_REQUIRE(workspace_bytes >= uav_groupnorm_workspace_bytes(n_outer, groups), "groupnorm from partials: workspace too small");
+  memset(prm, 0, sizeof(*prm));
+  int oct = 0;
+  int64_t min_bps = INT64_MAX;
+  for (int i = 0; i < n_sources; ++i) {
+    const uav_gn_source_t& sc = sources[i];
+    UAV_REQUIRE(sc.partial && sc.C > 0 && sc.C % 8 == 0 && sc.blocks > 0 && (sc.slabs == n_outer || sc.slabs == 1) &&
+                    sc.blocks % sc.slabs == 0,
+                "groupnorm from partials: bad source %d (C=%lld blocks=%lld slabs=%lld)", i, (long long)sc.C,
+                (long long)sc.blocks, (long long)sc.slabs);
+    prm->src[i].p = reinterpret_cast<const float2*>(sc.partial);
+    prm->src[i].blocks = sc.blocks;
+    prm->src[i].bps = sc.blocks / sc.slabs;
+    prm->src[i].slab_mul = sc.slabs == n_outer ? 1 : 0;
+    prm->src[i].oct0 = oct;
+    prm->src[i].octs = (int)(sc.C / 8);
+    oct += (int)(sc.C / 8);
+    if (prm->src[i].bps < min_bps) min_bps = prm->src[i].bps;
+  }
+  UAV_REQUIRE(oct * 8 == C, "groupnorm from partials: sources cover %d channels, x has %lld", oct * 8, (long long)C);
+  prm->nsrc = n_sources;
+  prm->oct_per_group = cpg / 8;
+  prm->G = groups;
+  // enough CTAs to pull the blocks at HBM speed, at least ~256 blocks per split; GN_MAX_SPLIT doubles fit the workspace
+  int64_t S = (4 * (int64_t)num_sms() + groups * n_outer - 1) / (groups * n_outer);
+  if (S > min_bps / 256) S = min_bps / 256;
+  if (S > GN_MAX_SPLIT) S = GN_MAX_SPLIT;
+  if (S < 1) S = 1;
+  *S_out = (int)S;
+  return UAV_OK;
+}
+
+// statistics stage from the producers' blocks, launch: fp64 reduction -> sums[n][g][S][2] at the head of `workspace`
+static uav_status_t gn_reduce_sources(const GnReduceParams& prm, int64_t n_outer, int S, void* workspace,
+                                      cudaStream_t stream) {
+  gn_reduce_partials_kernel<<<dim3((unsigned)prm.G, (unsigned)n_outer, (unsigned)S), 256, 0, stream>>>(
+      prm, reinterpret_cast<double*>(workspace));
+  GN_LAUNCHED();
+  return UAV_OK;
+}
+
+// apply stage, vector path: channels [chan, chan + Cs) of a C-channel GroupNorm from sums[n][g][S][2] at the head of
+// `workspace`.  x: 16-byte aligned fp16 rows of ld_in elements (Cs, ld_in, ld_out % 8 == 0), slab n at n * x_slab_stride.
+static uav_status_t gn_apply(const void* x, int64_t n_outer, int64_t pixels, int64_t Cs, int64_t ld_in,
+                             int64_t x_slab_stride, int groups, const void* workspace, int S, const float* gamma,
+                             const float* beta, float eps, int silu, void* y, int64_t ld_out, int64_t C, int chan,
+                             cudaStream_t stream) {
+  const int64_t gx = gn_blocks(16, n_outer, pixels, GN_THREADS / (Cs / 8) * 4);
+  gn_apply_vec_kernel<<<dim3((unsigned)gx, (unsigned)n_outer), GN_THREADS, 0, stream>>>(
+      reinterpret_cast<const __half*>(x), pixels, (int)Cs, ld_in, groups, reinterpret_cast<const double*>(workspace), S,
+      gamma, beta, eps, silu, reinterpret_cast<__half*>(y), ld_out, (int)C, chan, x_slab_stride);
+  GN_LAUNCHED();
+  return UAV_OK;
+}
+
 uav_status_t uav_groupnorm_silu(const void* x, int64_t n_outer, int64_t pixels, int64_t C,
                                 int64_t ld_in, int groups, const float* gamma, const float* beta,
                                 float eps, int silu, void* y, int64_t ld_out, void* workspace,
@@ -493,109 +542,18 @@ uav_status_t uav_groupnorm_silu(const void* x, int64_t n_outer, int64_t pixels, 
   UAV_REQUIRE(n_outer <= 65535, "uav_groupnorm_silu: n_outer too large");
   UAV_REQUIRE(workspace_bytes >= uav_groupnorm_workspace_bytes(n_outer, groups),
               "uav_groupnorm_silu: workspace too small");
-  double* sums = reinterpret_cast<double*>(workspace);
-  float2* partial = reinterpret_cast<float2*>(sums + n_outer * groups * 2);
-  const int cpg = (int)(C / groups);
-  const bool vec = (C % 8 == 0) && (cpg % 4 == 0) && (ld_in % 8 == 0) &&
-                   ((reinterpret_cast<uintptr_t>(x) & 15) == 0);
-  const int sms = num_sms();
-  int64_t gx;
-  if (vec) {
-    const int octs = (int)(C / 8);
-    const int pix_per_iter = GN_THREADS / octs;
-    int64_t want = (sms * 8 + n_outer - 1) / n_outer;
-    int64_t maxb = (pixels + pix_per_iter - 1) / pix_per_iter;
-    maxb = (maxb + 15) / 16;  // >= ~16 pixels per thread to amortise the block reduction
-    gx = want < maxb ? want : maxb;
-    if (gx < 1) gx = 1;
-    if (gx > GN_MAX_BLOCKS_PER_N) gx = GN_MAX_BLOCKS_PER_N;
-    gn_stats_kernel<<<dim3((unsigned)gx, (unsigned)n_outer), GN_THREADS, 0, stream>>>(
-        reinterpret_cast<const __half*>(x), pixels, (int)C, ld_in, groups, partial);
-  } else {
-    int64_t want = (sms * 4 + n_outer - 1) / n_outer;
-    int64_t maxb = (pixels + GN_THREADS - 1) / GN_THREADS;
-    gx = want < maxb ? want : maxb;
-    if (gx < 1) gx = 1;
-    if (gx > GN_MAX_BLOCKS_PER_N) gx = GN_MAX_BLOCKS_PER_N;
-    gn_stats_generic_kernel<<<dim3((unsigned)gx, (unsigned)n_outer), GN_THREADS, 0, stream>>>(
-        reinterpret_cast<const __half*>(x), pixels, (int)C, ld_in, groups, partial);
-  }
-  UAV_CHECK_CUDA(cudaGetLastError());
-  gn_finalize_kernel<<<dim3((unsigned)groups, (unsigned)n_outer), 256, 0, stream>>>(partial, (int)gx, groups,
-                                                                                              sums);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  {
-    const bool vec_apply = (C % 8 == 0) && (ld_in % 8 == 0) && (ld_out % 8 == 0) &&
-                           ((reinterpret_cast<uintptr_t>(x) & 15) == 0) &&
-                           ((reinterpret_cast<uintptr_t>(y) & 15) == 0);
-    UAV_REQUIRE(vec_apply || C % 8 != 0,
-                "uav_groupnorm_silu: C %% 8 == 0 tensors must be 16-byte aligned with ld %% 8 == 0");
-    if (vec_apply) {
-      const int octs = (int)(C / 8);
-      const int pix_per_iter = GN_THREADS / octs;
-      int64_t want = (sms * 16 + n_outer - 1) / n_outer;
-      int64_t maxb = (pixels + pix_per_iter * 4 - 1) / (pix_per_iter * 4);
-      int64_t gxa = want < maxb ? want : maxb;
-      if (gxa < 1) gxa = 1;
-      gn_apply_vec_kernel<<<dim3((unsigned)gxa, (unsigned)n_outer), GN_THREADS, 0, stream>>>(
-          reinterpret_cast<const __half*>(x), pixels, (int)C, ld_in, groups, sums, 1, gamma, beta, eps, silu,
-          reinterpret_cast<__half*>(y), ld_out, (int)C, 0, pixels * ld_in);
-    } else {
-      const int64_t work = pixels * C;
-      int64_t want = (sms * 16 + n_outer - 1) / n_outer;
-      int64_t maxb = (work + GN_THREADS * 4 - 1) / (GN_THREADS * 4);
-      int64_t gxa = want < maxb ? want : maxb;
-      if (gxa < 1) gxa = 1;
-      gn_apply_kernel<<<dim3((unsigned)gxa, (unsigned)n_outer), GN_THREADS, 2 * C * sizeof(float),
-                        stream>>>(reinterpret_cast<const __half*>(x), pixels, (int)C, ld_in, groups,
-                                  sums, gamma, beta, eps, silu, reinterpret_cast<__half*>(y),
-                                  ld_out);
-    }
-  }
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(3, std::memory_order_relaxed);
-  return UAV_OK;
-}
-
-// fp64 reduction of the producers' statistics blocks -> sums[n][g][S][2] at the head of `workspace`; returns S
-static uav_status_t gn_reduce_sources(int64_t n_outer, int64_t C, int groups, const uav_gn_source_t* sources, int n_sources,
-                                      void* workspace, size_t workspace_bytes, cudaStream_t stream, int* S_out) {
-  const int cpg = (int)(C / groups);
-  UAV_REQUIRE(cpg % 8 == 0, "groupnorm from partials: channels per group (%d) must be a multiple of 8", cpg);
-  UAV_REQUIRE(n_sources >= 1 && n_sources <= 4, "groupnorm from partials: 1..4 sources");
-  UAV_REQUIRE(workspace_bytes >= uav_groupnorm_workspace_bytes(n_outer, groups), "groupnorm from partials: workspace too small");
-  GnReduceParams prm;
-  memset(&prm, 0, sizeof(prm));
-  int oct = 0;
-  int64_t min_bps = INT64_MAX;
-  for (int i = 0; i < n_sources; ++i) {
-    const uav_gn_source_t& sc = sources[i];
-    UAV_REQUIRE(sc.partial && sc.C > 0 && sc.C % 8 == 0 && sc.blocks > 0 && (sc.slabs == n_outer || sc.slabs == 1) &&
-                    sc.blocks % sc.slabs == 0,
-                "groupnorm from partials: bad source %d (C=%lld blocks=%lld slabs=%lld)", i, (long long)sc.C,
-                (long long)sc.blocks, (long long)sc.slabs);
-    prm.src[i].p = reinterpret_cast<const float2*>(sc.partial);
-    prm.src[i].blocks = sc.blocks;
-    prm.src[i].bps = sc.blocks / sc.slabs;
-    prm.src[i].slab_mul = sc.slabs == n_outer ? 1 : 0;
-    prm.src[i].oct0 = oct;
-    prm.src[i].octs = (int)(sc.C / 8);
-    oct += (int)(sc.C / 8);
-    if (prm.src[i].bps < min_bps) min_bps = prm.src[i].bps;
-  }
-  UAV_REQUIRE(oct * 8 == C, "groupnorm from partials: sources cover %d channels, x has %lld", oct * 8, (long long)C);
-  prm.nsrc = n_sources;
-  prm.oct_per_group = cpg / 8;
-  prm.G = groups;
-  // enough CTAs to pull the blocks at HBM speed, at least ~256 blocks per split; GN_MAX_SPLIT doubles fit the workspace
-  int64_t S = (4 * (int64_t)num_sms() + groups * n_outer - 1) / (groups * n_outer);
-  if (S > min_bps / 256) S = min_bps / 256;
-  if (S > GN_MAX_SPLIT) S = GN_MAX_SPLIT;
-  if (S < 1) S = 1;
-  gn_reduce_partials_kernel<<<dim3((unsigned)groups, (unsigned)n_outer, (unsigned)S), 256, 0, stream>>>(
-      prm, reinterpret_cast<double*>(workspace));
-  UAV_CHECK_CUDA(cudaGetLastError());
-  *S_out = (int)S;
+  UAV_REQUIRE(C % 8 != 0 || (ld_in % 8 == 0 && ld_out % 8 == 0 && aligned16(x) && aligned16(y)),
+              "uav_groupnorm_silu: C %% 8 == 0 tensors must be 16-byte aligned with ld %% 8 == 0");
+  uav_status_t st = gn_stats_pass(x, n_outer, pixels, C, ld_in, groups, workspace, stream);
+  if (st != UAV_OK) return st;
+  if (C % 8 == 0)
+    return gn_apply(x, n_outer, pixels, C, ld_in, pixels * ld_in, groups, workspace, 1, gamma, beta, eps, silu, y, ld_out,
+                    C, 0, stream);
+  gn_apply_kernel<<<dim3((unsigned)gn_blocks(16, n_outer, pixels * C, GN_THREADS * 4), (unsigned)n_outer), GN_THREADS,
+                    2 * C * sizeof(float), stream>>>(reinterpret_cast<const __half*>(x), pixels, (int)C, ld_in, groups,
+                                                     reinterpret_cast<const double*>(workspace), gamma, beta, eps, silu,
+                                                     reinterpret_cast<__half*>(y), ld_out);
+  GN_LAUNCHED();
   return UAV_OK;
 }
 
@@ -607,38 +565,24 @@ uav_status_t uav_groupnorm_affine(const void* x, int64_t n_outer, int64_t pixels
   UAV_REQUIRE(gamma && beta && affine && workspace, "uav_groupnorm_affine: null pointer");
   UAV_REQUIRE(n_outer > 0 && n_outer <= 65535 && pixels > 0 && C > 0 && C <= 2048 && groups > 0 && C % groups == 0,
               "uav_groupnorm_affine: bad shape (C=%lld groups=%d)", (long long)C, groups);
-  double* sums = reinterpret_cast<double*>(workspace);
   int S = 1;
-  int launches = 2;
+  uav_status_t st;
   if (n_sources > 0) {
     UAV_REQUIRE(sources != nullptr, "uav_groupnorm_affine: null sources");
-    uav_status_t st = gn_reduce_sources(n_outer, C, groups, sources, n_sources, workspace, workspace_bytes, stream, &S);
-    if (st != UAV_OK) return st;
+    GnReduceParams prm;
+    st = gn_reduce_plan(n_outer, C, groups, sources, n_sources, workspace_bytes, &prm, &S);
+    if (st == UAV_OK) st = gn_reduce_sources(prm, n_outer, S, workspace, stream);
   } else {
-    UAV_REQUIRE(x != nullptr && ld_in >= C && C % 8 == 0 && (C / groups) % 4 == 0 && ld_in % 8 == 0 &&
-                    (reinterpret_cast<uintptr_t>(x) & 15) == 0,
+    UAV_REQUIRE(x != nullptr && ld_in >= C && C % 8 == 0 && (C / groups) % 4 == 0 && ld_in % 8 == 0 && aligned16(x),
                 "uav_groupnorm_affine: without sources x must be an aligned fp16 tensor with C %% 8 == 0");
     UAV_REQUIRE(workspace_bytes >= uav_groupnorm_workspace_bytes(n_outer, groups), "uav_groupnorm_affine: workspace too small");
-    float2* partial = reinterpret_cast<float2*>(sums + n_outer * groups * 2);
-    const int octs = (int)(C / 8);
-    const int pix_per_iter = GN_THREADS / octs;
-    int64_t want = ((int64_t)num_sms() * 8 + n_outer - 1) / n_outer;
-    int64_t maxb = ((pixels + pix_per_iter - 1) / pix_per_iter + 15) / 16;
-    int64_t gx = want < maxb ? want : maxb;
-    if (gx < 1) gx = 1;
-    if (gx > GN_MAX_BLOCKS_PER_N) gx = GN_MAX_BLOCKS_PER_N;
-    gn_stats_kernel<<<dim3((unsigned)gx, (unsigned)n_outer), GN_THREADS, 0, stream>>>(
-        reinterpret_cast<const __half*>(x), pixels, (int)C, ld_in, groups, partial);
-    UAV_CHECK_CUDA(cudaGetLastError());
-    gn_finalize_kernel<<<dim3((unsigned)groups, (unsigned)n_outer), 256, 0, stream>>>(partial, (int)gx, groups, sums);
-    UAV_CHECK_CUDA(cudaGetLastError());
-    launches = 3;
+    st = gn_stats_pass(x, n_outer, pixels, C, ld_in, groups, workspace, stream);
   }
+  if (st != UAV_OK) return st;
   gn_affine_kernel<<<dim3((unsigned)((C + 255) / 256), (unsigned)n_outer), 256, 0, stream>>>(
-      sums, S, groups, (int)C, static_cast<double>(pixels) * (C / groups), gamma, beta, eps,
-      reinterpret_cast<float2*>(affine));
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(launches, std::memory_order_relaxed);
+      reinterpret_cast<const double*>(workspace), S, groups, (int)C, static_cast<double>(pixels) * (C / groups), gamma,
+      beta, eps, reinterpret_cast<float2*>(affine));
+  GN_LAUNCHED();
   return UAV_OK;
 }
 
@@ -653,42 +597,34 @@ uav_status_t uav_groupnorm_silu_from_partials(const void* x, int64_t n_outer, in
   UAV_REQUIRE(n_outer > 0 && n_outer <= 65535 && pixels > 0 && C > 0 && C <= 2048 && groups > 0 && C % groups == 0 &&
                   ld_out >= C,
               "uav_groupnorm_silu_from_partials: bad shape (C=%lld groups=%d)", (long long)C, groups);
-  UAV_REQUIRE(C % 8 == 0 && (x == nullptr || (ld_in % 8 == 0 && ld_in >= C)) && ld_out % 8 == 0 &&
-                  (reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(y) & 15) == 0,
+  UAV_REQUIRE(C % 8 == 0 && (x == nullptr || (ld_in % 8 == 0 && ld_in >= C)) && ld_out % 8 == 0 && aligned16(x) &&
+                  aligned16(y),
               "uav_groupnorm_silu_from_partials: tensors must be 16-byte aligned with ld %% 8 == 0");
-  double* sums = reinterpret_cast<double*>(workspace);
+  GnReduceParams prm;
   int S = 1;
-  {
-    uav_status_t st = gn_reduce_sources(n_outer, C, groups, sources, n_sources, workspace, workspace_bytes, stream, &S);
-    if (st != UAV_OK) return st;
-  }
+  uav_status_t st = gn_reduce_plan(n_outer, C, groups, sources, n_sources, workspace_bytes, &prm, &S);
+  if (st != UAV_OK) return st;
   // apply: one launch over x, or — when the sources carry their own tensors (a concat that was never materialised) — one
   // launch per source, each writing its channel range of the dense output
   const bool per_source = sources[0].x != nullptr;
-  int launches = 1;
-  int chan = 0;
-  for (int i = 0; i < (per_source ? n_sources : 1); ++i) {
-    const int64_t Cs = per_source ? sources[i].C : C;
-    const __half* xs = reinterpret_cast<const __half*>(per_source ? sources[i].x : x);
-    const int64_t lds = per_source ? sources[i].ld : ld_in;
-    const int64_t slab_stride = per_source ? sources[i].slab_stride : pixels * ld_in;
-    if (per_source)
-      UAV_REQUIRE(xs != nullptr && lds >= Cs && lds % 8 == 0 && (reinterpret_cast<uintptr_t>(xs) & 15) == 0 && Cs <= 2048,
-                  "uav_groupnorm_silu_from_partials: bad tensor of source %d", i);
-    const int octs = (int)(Cs / 8);
-    const int pix_per_iter = GN_THREADS / octs;
-    int64_t want = ((int64_t)num_sms() * 16 + n_outer - 1) / n_outer;
-    int64_t maxb = (pixels + pix_per_iter * 4 - 1) / (pix_per_iter * 4);
-    int64_t gxa = want < maxb ? want : maxb;
-    if (gxa < 1) gxa = 1;
-    gn_apply_vec_kernel<<<dim3((unsigned)gxa, (unsigned)n_outer), GN_THREADS, 0, stream>>>(
-        xs, pixels, (int)Cs, lds, groups, sums, (int)S, gamma, beta, eps, silu, reinterpret_cast<__half*>(y), ld_out, (int)C,
-        chan, slab_stride);
-    UAV_CHECK_CUDA(cudaGetLastError());
-    chan += (int)Cs;
-    launches = 1 + i + 1;
+  for (int i = 0; per_source && i < n_sources; ++i) {
+    const uav_gn_source_t& sc = sources[i];
+    UAV_REQUIRE(sc.x != nullptr && sc.ld >= sc.C && sc.ld % 8 == 0 && aligned16(sc.x) && sc.C <= 2048,
+                "uav_groupnorm_silu_from_partials: bad tensor of source %d", i);
   }
-  g_launches.fetch_add(launches, std::memory_order_relaxed);
+  st = gn_reduce_sources(prm, n_outer, S, workspace, stream);
+  if (st != UAV_OK) return st;
+  if (!per_source)
+    return gn_apply(x, n_outer, pixels, C, ld_in, pixels * ld_in, groups, workspace, S, gamma, beta, eps, silu, y, ld_out,
+                    C, 0, stream);
+  int chan = 0;
+  for (int i = 0; i < n_sources; ++i) {
+    const uav_gn_source_t& sc = sources[i];
+    st = gn_apply(sc.x, n_outer, pixels, sc.C, sc.ld, sc.slab_stride, groups, workspace, S, gamma, beta, eps, silu, y,
+                  ld_out, C, chan, stream);
+    if (st != UAV_OK) return st;
+    chan += (int)sc.C;
+  }
   return UAV_OK;
 }
 

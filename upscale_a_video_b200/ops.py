@@ -292,13 +292,35 @@ def conv3d(x: torch.Tensor, w: torch.Tensor, bias=None, *, out=None, residual=No
 _gn_ws = {}
 
 
-def _gn_workspace(device, nbytes):
+def _gn_workspace(device, n_outer: int, groups: int):
+    """the GroupNorm scratch of the current stream, grown to uav_groupnorm_workspace_bytes(n_outer, groups)"""
+    nbytes = _lib.load().uav_groupnorm_workspace_bytes(n_outer, groups)
     key = (device, torch.cuda.current_stream().cuda_stream)
     ws = _gn_ws.get(key)
     if ws is None or ws.numel() < nbytes:
         ws = torch.empty(max(nbytes, 1 << 16), dtype=torch.uint8, device=device)
         _gn_ws[key] = ws
     return ws
+
+
+def _gn_sources(stats, C: int, groups: int, n_outer: int, batch: int, parts=None):
+    """ctypes uav_gn_source_t table of a C-channel GroupNorm over the channel concatenation whose parts' producers emitted
+    `stats` (one GnStats per part), or None when they cannot serve.  `parts`: the parts themselves, for a concatenation
+    that is never built (a batch-1 part serves every batch item)."""
+    if not (stats and (C // groups) % 8 == 0 and len(stats) <= 4 and sum(s.C for s in stats) == C):
+        return None
+    slabs = [s.slabs_for(n_outer, batch) for s in stats]
+    if not all(slabs):
+        return None
+    srcs = (_lib.GnSource * len(stats))()
+    for i, (s, sl) in enumerate(zip(stats, slabs)):
+        srcs[i].partial, srcs[i].blocks, srcs[i].C, srcs[i].slabs = s.partial.data_ptr(), s.blocks, s.C, sl
+        if parts is not None:
+            p = parts[i]
+            ld = _pixel_ld(p)
+            srcs[i].x, srcs[i].ld = p.data_ptr(), ld
+            srcs[i].slab_stride = p.numel() // p.shape[-1] // p.shape[0] * ld if p.shape[0] > 1 else 0
+    return srcs
 
 
 def group_norm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, groups: int, eps: float, *, silu: bool,
@@ -315,9 +337,8 @@ def group_norm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, groups:
     if out is None:
         out = torch.empty(x.shape, dtype=torch.float16, device=x.device)
     lib = _lib.load()
-    nbytes = lib.uav_groupnorm_workspace_bytes(n_outer, groups)
-    ws = _gn_workspace(x.device, nbytes)
-    srcs = _gn_sources(x, stats, groups, n_outer, x.shape[0] if batch is None else batch)
+    ws = _gn_workspace(x.device, n_outer, groups)
+    srcs = _gn_sources(stats, C, groups, n_outer, x.shape[0] if batch is None else batch)
     if srcs is not None:
         with _timed("groupnorm", 0.0, 2.0 * 2 * total_pix * C, f"gn(fused stats) {total_pix}px C{C}"):  # read + write
             _lib.check(lib.uav_groupnorm_silu_from_partials(x.data_ptr(), n_outer, pixels, C, _pixel_ld(x), groups,
@@ -340,51 +361,27 @@ def group_norm_cat(parts, gamma: torch.Tensor, beta: torch.Tensor, groups: int, 
     misaligned slabs): the caller then materialises the concat."""
     B = max(p.shape[0] for p in parts)
     C = sum(p.shape[-1] for p in parts)
-    if (C // groups) % 8 or len(parts) > 4 or n_outer != B:
-        return None
-    lead = None
-    srcs = (_lib.GnSource * len(parts))()
-    for i, p in enumerate(parts):
+    lead = tuple(parts[0].shape[1:-1])
+    stats = []
+    for p in parts:
         st = getattr(p, "uav_gn", None)
-        if not st or len(st) != 1 or st[0].C != p.shape[-1] or p.dtype != torch.float16 or p.shape[0] not in (1, B):
+        if (not st or len(st) != 1 or st[0].C != p.shape[-1] or p.dtype != torch.float16 or p.shape[0] not in (1, B)
+                or tuple(p.shape[1:-1]) != lead):
             return None
-        sl = st[0].slabs_for(n_outer, B)
-        if not sl:
-            return None
-        if lead is None:
-            lead = tuple(p.shape[1:-1])
-        if tuple(p.shape[1:-1]) != lead:
-            return None
-        ld = _pixel_ld(p)
-        pix = p.numel() // p.shape[-1] // p.shape[0]
-        srcs[i].partial, srcs[i].blocks, srcs[i].C, srcs[i].slabs = st[0].partial.data_ptr(), st[0].blocks, st[0].C, sl
-        srcs[i].x, srcs[i].ld, srcs[i].slab_stride = p.data_ptr(), ld, (pix * ld if p.shape[0] == B and B > 1 else 0)
-        if B == 1:
-            srcs[i].slab_stride = 0
+        stats.append(st[0])
+    srcs = _gn_sources(stats, C, groups, n_outer, B, parts) if n_outer == B else None
+    if srcs is None:
+        return None
     out = torch.empty(B, *lead, C, dtype=torch.float16, device=parts[0].device)
     pixels = out.numel() // C // n_outer
     lib = _lib.load()
-    ws = _gn_workspace(out.device, lib.uav_groupnorm_workspace_bytes(n_outer, groups))
+    ws = _gn_workspace(out.device, n_outer, groups)
     with _timed("groupnorm", 0.0, 2.0 * 2 * out.numel(), f"gn(virtual concat) {out.numel() // C}px C{C}"):
         _lib.check(lib.uav_groupnorm_silu_from_partials(None, n_outer, pixels, C, C, groups, gamma.data_ptr(), beta.data_ptr(),
                                                         eps, 1 if silu else 0, out.data_ptr(), C, srcs, len(parts),
                                                         ws.data_ptr(), ws.numel(), _stream()),
                    "uav_groupnorm_silu_from_partials")
     return out
-
-
-def _gn_sources(x, stats, groups: int, n_outer: int, batch: int):
-    """ctypes source table for a tensor whose producer(s) emitted GroupNorm statistics, or None"""
-    C = x.shape[-1]
-    if not (stats and (C // groups) % 8 == 0 and len(stats) <= 4 and sum(s.C for s in stats) == C):
-        return None
-    slabs = [s.slabs_for(n_outer, batch) for s in stats]
-    if not all(slabs):
-        return None
-    srcs = (_lib.GnSource * len(stats))()
-    for i, (s, sl) in enumerate(zip(stats, slabs)):
-        srcs[i].partial, srcs[i].blocks, srcs[i].C, srcs[i].slabs = s.partial.data_ptr(), s.blocks, s.C, sl
-    return srcs
 
 
 def conv_out_fused(x: torch.Tensor, gamma, beta, groups: int, eps: float, w: torch.Tensor, bias, cout: int, out_dtype,
@@ -397,10 +394,10 @@ def conv_out_fused(x: torch.Tensor, gamma, beta, groups: int, eps: float, w: tor
     B, T, H, W, Cc = x.shape
     assert x.dtype == torch.float16 and w.dtype == torch.float16 and w.is_contiguous() and tuple(w.shape[1:]) == (3, 3, Cc)
     lib = _lib.load()
-    ws = _gn_workspace(x.device, lib.uav_groupnorm_workspace_bytes(B, groups))
+    ws = _gn_workspace(x.device, B, groups)
     affine = torch.empty(B, Cc, 2, dtype=torch.float32, device=x.device)
     stats = getattr(x, "uav_gn", None)
-    srcs = _gn_sources(x, stats, groups, B, B)
+    srcs = _gn_sources(stats, Cc, groups, B, B)
     with _timed("groupnorm", 0.0, 2.0 * x.numel() if srcs is None else 0.0, f"gn affine {x.numel() // Cc}px C{Cc}"):
         _lib.check(lib.uav_groupnorm_affine(x.data_ptr(), B, T * H * W, Cc, _pixel_ld(x), groups, gamma.data_ptr(),
                                             beta.data_ptr(), eps, srcs, 0 if srcs is None else len(stats),
