@@ -240,7 +240,7 @@ uav_status_t uav_layernorm(const void* x, int64_t rows, int64_t C, int64_t ld_in
  * q [batch][nq][ldq], k/v [batch / kv_batch_div][nk][ld], out [batch][nq][ldo]; head h occupies
  * columns [h*head_dim, (h+1)*head_dim).  kv_batch_div = frames when the text K/V are shared by all
  * frames of a batch item (the reference repeats them: attention.py:364).  head_dim 64, 128, or
- * 512 (single head). */
+ * 512 (single head).  q, k, v and out must be 16-byte aligned. */
 uav_status_t uav_attention(const void* q, const void* k, const void* v, void* out, int64_t batch,
                            int heads, int head_dim, int64_t nq, int64_t nk, int64_t ldq,
                            int64_t ldk, int64_t ldv, int64_t ldo, int64_t kv_batch_div,
@@ -250,8 +250,9 @@ uav_status_t uav_attention(const void* q, const void* k, const void* v, void* ou
  * q is scaled, q and k get the rotary embedding on dims [0,32) (cos/sin table rot[F][16][2]),
  * scores += rel_bias[heads][F][F], row-max subtract, softmax, PV.  Tokens are ordered
  * (b, f, hw) — the channels-last video layout — so no rearrange copies are needed.  head_dim 64
- * or 128.  F <= 8 runs on the windowed-pipeline kernels; F > 8 on an online-softmax kernel that
- * streams 16-frame key tiles. */
+ * or 128.  q, k, v, out and rot_cos_sin must be 16-byte aligned.  F <= 8 with an even head count
+ * runs on the windowed-pipeline kernel; everything else on an online-softmax kernel that streams
+ * 16-frame key tiles. */
 uav_status_t uav_temporal_attention(const void* q, const void* k, const void* v, void* out,
                                     int64_t B, int64_t F, int64_t HW, int heads, int head_dim,
                                     int64_t ldq, int64_t ldk, int64_t ldv, int64_t ldo,

@@ -150,6 +150,34 @@ def test_groupnorm_validates_before_launch(uav_lib):
     assert uav_lib.uav_launch_count() == 0
 
 
+def test_attention_validates_before_launch(uav_lib):
+    """uav_attention and uav_temporal_attention run all their checks before they opt in or launch: a bad call returns
+    its status and message and launches nothing, on every kernel path (cross, flash, wgmma, temporal).  The pointers are
+    never dereferenced."""
+    A, M = 1 << 20, (1 << 20) + 8  # 16-byte aligned and misaligned fake pointers
+
+    def attention(q=A, k=A, v=A, out=A, batch=1, heads=8, d=64, nq=4096, nk=77):
+        C = heads * d
+        return uav_lib.uav_attention(q, k, v, out, batch, heads, d, nq, nk, C, C, C, C, 1, 0.125, None)
+
+    def temporal(q=A, rot=A, d=64, F=4):
+        C = 8 * d
+        return uav_lib.uav_temporal_attention(q, A, A, A, 1, F, 16, 8, d, C, C, C, C, 0.125, rot, A, None)
+
+    def rejects(st, msg, status=1):
+        assert st == status and msg in uav_lib.uav_last_error_string(), (st, msg, uav_lib.uav_last_error_string())
+
+    rejects(attention(q=M), b"uav_attention: q must be 16-byte aligned")
+    rejects(attention(out=M), b"uav_attention: out must be 16-byte aligned")
+    rejects(attention(k=M, nk=300), b"uav_attention: k must be 16-byte aligned")
+    rejects(attention(nq=(1 << 31) + 64), b"uav_attention: nq or nk too large")
+    rejects(attention(heads=2, d=512, nq=1024, nk=1024), b"uav_attention: head_dim 512 supports a single head")
+    rejects(temporal(q=M), b"uav_temporal_attention: q must be 16-byte aligned")
+    rejects(temporal(rot=M), b"uav_temporal_attention: rot_cos_sin must be 16-byte aligned")
+    rejects(temporal(d=96), b"uav_temporal_attention: head_dim 96 unsupported", status=3)
+    assert uav_lib.uav_launch_count() == 0
+
+
 def test_scheduler_host_tables_match_oracle():
     """DDIMScheduler's host-side schedule (timesteps, alphas) is plain CPU math: compare with the oracle without a GPU"""
     import json

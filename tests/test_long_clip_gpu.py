@@ -109,12 +109,14 @@ def _kernels_run(fn):
 
 
 def test_temporal_attention_kernel_selection():
-    """F > 8 runs the online-softmax kernel; F <= 8 keeps the mma kernel of the pipeline's windows"""
+    """F > 8 or an odd head count runs the online-softmax kernel; F <= 8 with an even head count keeps the mma kernel of
+    the pipeline's windows"""
     from upscale_a_video_b200 import ops
-    for Fr, want, other in ((12, "temporal_attn_long_kernel", "temporal_attn_mma_kernel"),
-                            (8, "temporal_attn_mma_kernel", "temporal_attn_long_kernel")):
-        q, k, v, _, rot, bias = _temporal_inputs(1, Fr, 40, 8, 64)
-        names = _kernels_run(lambda: ops.temporal_attention(q, k, v, 8, rot, bias))
+    for Fr, heads, want, other in ((12, 8, "temporal_attn_long_kernel", "temporal_attn_mma_kernel"),
+                                   (8, 8, "temporal_attn_mma_kernel", "temporal_attn_long_kernel"),
+                                   (4, 3, "temporal_attn_long_kernel", "temporal_attn_mma_kernel")):
+        q, k, v, _, rot, bias = _temporal_inputs(1, Fr, 40, heads, 64)
+        names = _kernels_run(lambda: ops.temporal_attention(q, k, v, heads, rot, bias))
         assert any(want in n for n in names) and not any(other in n for n in names), (Fr, names)
 
 

@@ -117,7 +117,7 @@ def test_attention_fused_qkv_slices():
 
 @pytest.mark.parametrize("B,Fr,HW,heads,d", [(2, 8, 96, 8, 64), (1, 3, 50, 8, 128), (2, 1, 33, 8, 64), (1, 5, 7, 8, 128),
                                              (1, 8, 2881, 8, 64), (2, 7, 19, 2, 128),
-                                             (1, 4, 10, 3, 64)])  # odd head count: shuffle kernel
+                                             (1, 4, 10, 3, 64)])  # odd head count: online-softmax kernel
 def test_temporal_attention(B, Fr, HW, heads, d):
     """vs the oracle's TemporalAttention restatement (attention.py:699-733) in fp32"""
     from oracle import uav_oracle as O

@@ -9,18 +9,86 @@
 //    kernel (fp16 in, fp32 accumulate, fp32 online softmax).
 //  * uav_temporal_attention: the seq = T per-pixel attention with rotary embedding on the
 //    first 32 dims and the T5-style relative-position bias (attention.py:699-733).  T <= 8 (the
-//    pipeline's windows) runs on an mma.sync kernel for a pair of heads, or on a register-resident
-//    warp kernel for an odd head count: one warp per (pixel, head), lane = (frame, quarter of the
-//    head dim), K/V exchanged with warp shuffles.  T > 8 runs on an mma.sync kernel with an
-//    online softmax over 16-frame key tiles.  All read q/k/v in the (b, f, hw, c) layout, so the
-//    reference's two "(b f) d c <-> (b d) f c" rearrange copies (attention.py:555,560) do not
-//    exist.
+//    pipeline's windows) with an even head count runs on an mma.sync kernel for a pair of heads;
+//    every other case runs on an mma.sync kernel for one head with an online softmax over
+//    16-frame key tiles.  Both read q/k/v in the (b, f, hw, c) layout, so the reference's two
+//    "(b f) d c <-> (b d) f c" rearrange copies (attention.py:555,560) do not exist.
+//
+// All four kernels are built from the warp-tile helpers below: S = Q K^T, the P fragment, O += P V and the output
+// staging are written once.
 #include "uav_common.cuh"
 
 #include <atomic>
 
 namespace uav {
 extern std::atomic<uint64_t> g_launches;
+
+// ---------------------------------------------------------------------------------------
+// warp tiles: a warp owns 16 query rows.  Lane l holds rows l / 4 and l / 4 + 8 of every 16 x 8 accumulator block,
+// columns 2 (l % 4) + {0, 1} (mma16816).  Q, K and V are tile_ptr<D> tiles of D halfs per row.
+// ---------------------------------------------------------------------------------------
+// s[n] += Q K^T for keys [8 n, 8 n + 8): the 16 Q rows of sQ from which the lane loads row arow (row0 + (lane & 7) +
+// 8 ((lane >> 3) & 1)), key rows [0, 16 NB16) of sK, over the k-steps of 16 dims [KK_BEGIN, D / 16)
+template <int D, int NB16, int KK_BEGIN = 0>
+__device__ __forceinline__ void warp_qk(float (&s)[NB16 * 2][4], __half* sQ, int arow, __half* sK, int lane) {
+  const int brow = (lane & 7) + (lane >> 4) * 8, bchk = (lane >> 3) & 1;
+#pragma unroll
+  for (int kk = KK_BEGIN; kk < D / 16; ++kk) {
+    uint32_t a[4];
+    ldmatrix_x4(a, tile_ptr<D>(sQ, arow, kk * 2 + (lane >> 4)));
+#pragma unroll
+    for (int nb = 0; nb < NB16; ++nb) {
+      uint32_t bfr[4];
+      ldmatrix_x4(bfr, tile_ptr<D>(sK, nb * 16 + brow, kk * 2 + bchk));
+      mma16816(s[nb * 2], a, bfr[0], bfr[1]);
+      mma16816(s[nb * 2 + 1], a, bfr[2], bfr[3]);
+    }
+  }
+}
+
+// P of the accumulator block of keys [8 j, 8 j + 8) of a k16 step (p0, p1: row lane / 4; p2, p3: row lane / 4 + 8) ->
+// its half of the step's A fragment
+__device__ __forceinline__ void pack_p(uint32_t (&a)[4], int j, float p0, float p1, float p2, float p3) {
+  a[2 * j] = pack_half2_rn(p0, p1);
+  a[2 * j + 1] = pack_half2_rn(p2, p3);
+}
+
+// o[n] += P V for output columns [8 n, 8 n + 8): a is P of the 16 keys at rows [krow, krow + 16) of sV
+template <int D>
+__device__ __forceinline__ void warp_pv(float (&o)[D / 8][4], const uint32_t (&a)[4], __half* sV, int krow, int lane) {
+  const int vrow = krow + (lane & 7) + ((lane >> 3) & 1) * 8;
+#pragma unroll
+  for (int nb = 0; nb < D / 16; ++nb) {
+    uint32_t bfr[4];
+    ldmatrix_x4_trans(bfr, tile_ptr<D>(sV, vrow, nb * 2 + (lane >> 4)));
+    mma16816(o[nb * 2], a, bfr[0], bfr[1]);
+    mma16816(o[nb * 2 + 1], a, bfr[2], bfr[3]);
+  }
+}
+
+// max / sum over the 4 lanes of a quad, which together hold one accumulator row.  The temporal kernels reduce their
+// two rows with the shuffles interleaved instead.
+__device__ __forceinline__ float quad_max(float x) {
+  x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 1));
+  return fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 2));
+}
+__device__ __forceinline__ float quad_sum(float x) {
+  x += __shfl_xor_sync(0xffffffffu, x, 1);
+  return x + __shfl_xor_sync(0xffffffffu, x, 2);
+}
+
+// fp16 of the lane's accumulator rows times i0 (tile row r0) and i1 (tile row r0 + 8), t4 = lane % 4
+template <int D>
+__device__ __forceinline__ void stage_rows(__half* tile, int r0, const float (&o)[D / 8][4], float i0, float i1,
+                                           int t4) {
+#pragma unroll
+  for (int n = 0; n < D / 8; ++n) {
+    const __half2 v0 = __floats2half2_rn(o[n][0] * i0, o[n][1] * i0);
+    const __half2 v1 = __floats2half2_rn(o[n][2] * i1, o[n][3] * i1);
+    *reinterpret_cast<__half2*>(tile_ptr<D>(tile, r0, n) + t4 * 2) = v0;
+    *reinterpret_cast<__half2*>(tile_ptr<D>(tile, r0 + 8, n) + t4 * 2) = v1;
+  }
+}
 
 // ---------------------------------------------------------------------------------------
 // flash attention (mma.sync), d = 64
@@ -40,44 +108,6 @@ struct FaParams {
   int nq, nk, heads, kv_batch_div;
   float scale_log2;                  // softmax scale * log2(e)
 };
-
-__device__ __forceinline__ void cp_async16(void* smem, const void* gmem, bool valid) {
-  const uint32_t s = smem_u32(smem);
-  const int sz = valid ? 16 : 0;
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(s), "l"(gmem), "r"(sz)
-               : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() {
-  asm volatile("cp.async.commit_group;" ::: "memory");
-}
-template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
-}
-__device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], const void* p) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-               : "r"(smem_u32(p)));
-}
-__device__ __forceinline__ void ldmatrix_x4_trans(uint32_t (&r)[4], const void* p) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-               : "r"(smem_u32(p)));
-}
-__device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0,
-                                         uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, "
-      "{%0,%1,%2,%3};"
-      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
-// smem tile: rows of DT halfs, 16-byte chunks XOR-swizzled by (row & 7)
-template <int DT>
-__device__ __forceinline__ __half* tile_ptr(__half* base, int row, int chunk) {
-  return base + row * DT + ((chunk ^ (row & 7)) << 3);
-}
 
 __global__ void __launch_bounds__(FA_THREADS)
     flash_attn_kernel(const FaParams p) {
@@ -131,35 +161,20 @@ __global__ void __launch_bounds__(FA_THREADS)
 
   const int g = lane >> 2, t4 = lane & 3;
   const int arow = warp * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;  // ldmatrix A row
-  const int achk = lane >> 4;
-
   for (int tile = 0; tile < ntiles; ++tile) {
     const int buf = tile & 1;
     if (tile + 1 < ntiles) load_kv(tile + 1, buf ^ 1);
     cp_async_commit();
     cp_async_wait<1>();
     __syncthreads();
-    const __half* skb = sk + buf * FA_BN * FA_D;
-    const __half* svb = sv + buf * FA_BN * FA_D;
+    __half* skb = sk + buf * FA_BN * FA_D;
+    __half* svb = sv + buf * FA_BN * FA_D;
 
     // ---- S = Q K^T (16 x 64 per warp) ----
     float s[FA_BN / 8][4];
 #pragma unroll
     for (int i = 0; i < FA_BN / 8; ++i) s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f;
-#pragma unroll
-    for (int kk = 0; kk < FA_D / 16; ++kk) {
-      uint32_t a[4];
-      ldmatrix_x4(a, tile_ptr<FA_D>(sq, arow, kk * 2 + achk));
-#pragma unroll
-      for (int nb = 0; nb < FA_BN / 16; ++nb) {
-        uint32_t bfr[4];
-        const int brow = nb * 16 + (lane & 7) + (lane >> 4) * 8;
-        const int bchk = kk * 2 + ((lane >> 3) & 1);
-        ldmatrix_x4(bfr, tile_ptr<FA_D>(const_cast<__half*>(skb), brow, bchk));
-        mma16816(s[nb * 2], a, bfr[0], bfr[1]);
-        mma16816(s[nb * 2 + 1], a, bfr[2], bfr[3]);
-      }
-    }
+    warp_qk<FA_D, FA_BN / 16>(s, sq, arow, skb, lane);
     // ---- mask + online softmax (rows g and g+8 of this warp's 16) ----
     const int kbase = tile * FA_BN;
     float mx[2] = {-INFINITY, -INFINITY};
@@ -175,10 +190,7 @@ __global__ void __launch_bounds__(FA_THREADS)
       }
     }
 #pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffff, mx[r], 1));
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffff, mx[r], 2));
-    }
+    for (int r = 0; r < 2; ++r) mx[r] = quad_max(mx[r]);
     float corr[2], rs[2] = {0.f, 0.f};
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
@@ -186,16 +198,14 @@ __global__ void __launch_bounds__(FA_THREADS)
       corr[r] = (m_run[r] == -INFINITY) ? 0.f : exp2f(m_run[r] - mnew);
       m_run[r] = mnew;
     }
-    uint32_t pf[FA_BN / 8][2];  // P as fp16 pairs (A fragments)
+    uint32_t pf[FA_BN / 16][4];  // P as the A fragments of the k16 steps
 #pragma unroll
     for (int nb = 0; nb < FA_BN / 8; ++nb) {
       const float p0 = exp2f(s[nb][0] - m_run[0]), p1 = exp2f(s[nb][1] - m_run[0]);
       const float p2 = exp2f(s[nb][2] - m_run[1]), p3 = exp2f(s[nb][3] - m_run[1]);
       rs[0] += p0 + p1;
       rs[1] += p2 + p3;
-      __half2 h01 = __floats2half2_rn(p0, p1), h23 = __floats2half2_rn(p2, p3);
-      pf[nb][0] = *reinterpret_cast<uint32_t*>(&h01);
-      pf[nb][1] = *reinterpret_cast<uint32_t*>(&h23);
+      pack_p(pf[nb >> 1], nb & 1, p0, p1, p2, p3);
     }
 #pragma unroll
     for (int r = 0; r < 2; ++r) l_run[r] = l_run[r] * corr[r] + rs[r];
@@ -208,18 +218,7 @@ __global__ void __launch_bounds__(FA_THREADS)
     }
     // ---- O += P V ----
 #pragma unroll
-    for (int kk = 0; kk < FA_BN / 16; ++kk) {
-      const uint32_t a[4] = {pf[kk * 2][0], pf[kk * 2][1], pf[kk * 2 + 1][0], pf[kk * 2 + 1][1]};
-#pragma unroll
-      for (int nb = 0; nb < FA_D / 16; ++nb) {
-        uint32_t bfr[4];
-        const int vrow = kk * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
-        const int vchk = nb * 2 + (lane >> 4);
-        ldmatrix_x4_trans(bfr, tile_ptr<FA_D>(const_cast<__half*>(svb), vrow, vchk));
-        mma16816(o_acc[nb * 2], a, bfr[0], bfr[1]);
-        mma16816(o_acc[nb * 2 + 1], a, bfr[2], bfr[3]);
-      }
-    }
+    for (int kk = 0; kk < FA_BN / 16; ++kk) warp_pv<FA_D>(o_acc, pf[kk], svb, kk * 16, lane);
     __syncthreads();  // all warps done with buf before it is refilled
   }
   cp_async_wait<0>();
@@ -227,20 +226,11 @@ __global__ void __launch_bounds__(FA_THREADS)
   // ---- finalize: O / l -> smem (reuse Q tile region) -> coalesced stores ----
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
-    float l = l_run[r];
-    l += __shfl_xor_sync(0xffffffff, l, 1);
-    l += __shfl_xor_sync(0xffffffff, l, 2);
+    const float l = quad_sum(l_run[r]);
     l_run[r] = (l > 0.f) ? 1.f / l : 0.f;
   }
   __half* so = sq;  // [64][FA_D]
-#pragma unroll
-  for (int nb = 0; nb < FA_D / 8; ++nb) {
-    const int r0 = warp * 16 + g, r1 = r0 + 8;
-    __half2 v0 = __floats2half2_rn(o_acc[nb][0] * l_run[0], o_acc[nb][1] * l_run[0]);
-    __half2 v1 = __floats2half2_rn(o_acc[nb][2] * l_run[1], o_acc[nb][3] * l_run[1]);
-    *reinterpret_cast<__half2*>(tile_ptr<FA_D>(so, r0, nb) + t4 * 2) = v0;
-    *reinterpret_cast<__half2*>(tile_ptr<FA_D>(so, r1, nb) + t4 * 2) = v1;
-  }
+  stage_rows<FA_D>(so, warp * 16 + g, o_acc, l_run[0], l_run[1], t4);
   __syncthreads();
   for (int i = tid; i < FA_BM * QC; i += FA_THREADS) {
     const int r = i / QC, c = i % QC;
@@ -298,7 +288,6 @@ __global__ void __launch_bounds__(FA_THREADS)
 
   const int g = lane >> 2, t4 = lane & 3;
   const int arow = warp * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
-  const int achk = lane >> 4;
   int it = 0;
   for (; tile < ntiles; tile += tile_stride, ++it) {
     const int buf = it & 1;
@@ -313,20 +302,7 @@ __global__ void __launch_bounds__(FA_THREADS)
     float s[NB16 * 2][4];
 #pragma unroll
     for (int i = 0; i < NB16 * 2; ++i) s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f;
-#pragma unroll
-    for (int kk = 0; kk < D / 16; ++kk) {
-      uint32_t a[4];
-      ldmatrix_x4(a, tile_ptr<D>(sqb, arow, kk * 2 + achk));
-#pragma unroll
-      for (int nb = 0; nb < NB16; ++nb) {
-        uint32_t bfr[4];
-        const int brow = nb * 16 + (lane & 7) + (lane >> 4) * 8;
-        const int bchk = kk * 2 + ((lane >> 3) & 1);
-        ldmatrix_x4(bfr, tile_ptr<D>(sk, brow, bchk));
-        mma16816(s[nb * 2], a, bfr[0], bfr[1]);
-        mma16816(s[nb * 2 + 1], a, bfr[2], bfr[3]);
-      }
-    }
+    warp_qk<D, NB16>(s, sqb, arow, sk, lane);
     // row maxima of the raw scores (scale > 0); only 8-column blocks past nk hold padded keys
     float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
@@ -341,13 +317,9 @@ __global__ void __launch_bounds__(FA_THREADS)
       }
     }
 #pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffff, mx[r], 1));
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffff, mx[r], 2));
-      mx[r] *= p.scale_log2;
-    }
+    for (int r = 0; r < 2; ++r) mx[r] = quad_max(mx[r]) * p.scale_log2;
     float rs[2] = {0.f, 0.f};
-    uint32_t pf[NB16 * 2][2];
+    uint32_t pf[NB16][4];  // P as the A fragments of the k16 steps
 #pragma unroll
     for (int nb = 0; nb < NB16 * 2; ++nb) {
       // exp2(s * scale - max): one FFMA + one MUFU per score
@@ -355,43 +327,19 @@ __global__ void __launch_bounds__(FA_THREADS)
       const float p2 = ex2_ftz(fmaf(s[nb][2], p.scale_log2, -mx[1])), p3 = ex2_ftz(fmaf(s[nb][3], p.scale_log2, -mx[1]));
       rs[0] += p0 + p1;
       rs[1] += p2 + p3;
-      __half2 h01 = __floats2half2_rn(p0, p1), h23 = __floats2half2_rn(p2, p3);
-      pf[nb][0] = *reinterpret_cast<uint32_t*>(&h01);
-      pf[nb][1] = *reinterpret_cast<uint32_t*>(&h23);
+      pack_p(pf[nb >> 1], nb & 1, p0, p1, p2, p3);
     }
 #pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      rs[r] += __shfl_xor_sync(0xffffffff, rs[r], 1);
-      rs[r] += __shfl_xor_sync(0xffffffff, rs[r], 2);
-      rs[r] = 1.f / rs[r];
-    }
+    for (int r = 0; r < 2; ++r) rs[r] = 1.f / quad_sum(rs[r]);
     // O = P V
     float o_acc[D / 8][4];
 #pragma unroll
     for (int i = 0; i < D / 8; ++i) o_acc[i][0] = o_acc[i][1] = o_acc[i][2] = o_acc[i][3] = 0.f;
 #pragma unroll
-    for (int kk = 0; kk < NB16; ++kk) {
-      const uint32_t a[4] = {pf[kk * 2][0], pf[kk * 2][1], pf[kk * 2 + 1][0], pf[kk * 2 + 1][1]};
-#pragma unroll
-      for (int nb = 0; nb < D / 16; ++nb) {
-        uint32_t bfr[4];
-        const int vrow = kk * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
-        const int vchk = nb * 2 + (lane >> 4);
-        ldmatrix_x4_trans(bfr, tile_ptr<D>(sv, vrow, vchk));
-        mma16816(o_acc[nb * 2], a, bfr[0], bfr[1]);
-        mma16816(o_acc[nb * 2 + 1], a, bfr[2], bfr[3]);
-      }
-    }
+    for (int kk = 0; kk < NB16; ++kk) warp_pv<D>(o_acc, pf[kk], sv, kk * 16, lane);
     // stage this warp's 16 rows in its own (already consumed) rows of the Q buffer, then 16-byte stores
     __syncwarp();
-#pragma unroll
-    for (int nb = 0; nb < D / 8; ++nb) {
-      const int r0 = warp * 16 + g, r1 = r0 + 8;
-      __half2 v0 = __floats2half2_rn(o_acc[nb][0] * rs[0], o_acc[nb][1] * rs[0]);
-      __half2 v1 = __floats2half2_rn(o_acc[nb][2] * rs[1], o_acc[nb][3] * rs[1]);
-      *reinterpret_cast<__half2*>(tile_ptr<D>(sqb, r0, nb) + t4 * 2) = v0;
-      *reinterpret_cast<__half2*>(tile_ptr<D>(sqb, r1, nb) + t4 * 2) = v1;
-    }
+    stage_rows<D>(sqb, warp * 16 + g, o_acc, rs[0], rs[1], t4);
     __syncwarp();
     const int q0 = tile * FA_BM;
     for (int i = lane; i < 16 * QC; i += 32) {
@@ -405,25 +353,9 @@ __global__ void __launch_bounds__(FA_THREADS)
   cp_async_wait<0>();
 }
 
-template <int D, int NB16>
-static uav_status_t launch_cross(const FaParams& p, int batch, cudaStream_t stream) {
-  constexpr int smem = (2 * NB16 * 16 * D + 2 * FA_BM * D) * 2;
-  const uav_status_t st = opt_in_smem<cross_attn_kernel<D, NB16>>(smem);
-  if (st != UAV_OK) return st;
-  const int ntiles = (p.nq + FA_BM - 1) / FA_BM;
-  // enough CTAs to fill the GPU ~4x over, each streaming several query tiles past its resident K/V
-  int gx = (num_sms() * 8 + batch * p.heads - 1) / (batch * p.heads);
-  if (gx > ntiles) gx = ntiles;
-  if (gx < 1) gx = 1;
-  dim3 grid(gx * p.heads, batch);
-  cross_attn_kernel<D, NB16><<<grid, FA_THREADS, smem, stream>>>(p);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  return UAV_OK;
-}
-
 // ---------------------------------------------------------------------------------------
-// temporal attention: one warp per (batch, pixel, head); lane = frame * 4 + quarter
+// temporal attention: one warp per (batch, pixel) and one head (temporal_attn_long_kernel) or a pair of heads
+// (temporal_attn_mma_kernel)
 // ---------------------------------------------------------------------------------------
 struct TaParams {
   const __half* q;
@@ -438,135 +370,15 @@ struct TaParams {
   const float* bias;  // [heads][F][F]
 };
 
-template <int D>
-__global__ void __launch_bounds__(256)
-    temporal_attn_kernel(const TaParams p) {
-  constexpr int DP = D / 4;   // dims per lane
-  constexpr int HP = DP / 2;  // half2 per lane
-  const int lane = threadIdx.x & 31;
-  const int64_t wid = static_cast<int64_t>(blockIdx.x) * 8 + (threadIdx.x >> 5);
-  const int64_t total = static_cast<int64_t>(p.B) * p.HW * p.heads;
-  if (wid >= total) return;
-  const int h = static_cast<int>(wid % p.heads);
-  const int64_t pix = (wid / p.heads) % p.HW;
-  const int b = static_cast<int>(wid / (p.heads * p.HW));
-  const int i = lane >> 2, part = lane & 3;
-  const bool act = i < p.F;
-  const int64_t tok = (static_cast<int64_t>(b) * p.F + (act ? i : 0)) * p.HW + pix;
-  const int off = h * D + part * DP;
-
-  float qf[DP];
-  __half2 kh[HP], vh[HP];
-  {
-    const __half* qp = p.q + tok * p.ldq + off;
-    const __half* kp = p.k + tok * p.ldk + off;
-    const __half* vp = p.v + tok * p.ldv + off;
-#pragma unroll
-    for (int c = 0; c < DP / 8; ++c) {
-      const uint4 a = act ? ldg16(qp + c * 8) : make_uint4(0, 0, 0, 0);
-      const uint4 bq = act ? ldg16(kp + c * 8) : make_uint4(0, 0, 0, 0);
-      const uint4 cq = act ? ldg16(vp + c * 8) : make_uint4(0, 0, 0, 0);
-      const __half2* ah = reinterpret_cast<const __half2*>(&a);
-      const __half2* bh = reinterpret_cast<const __half2*>(&bq);
-      const __half2* ch = reinterpret_cast<const __half2*>(&cq);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 f = __half22float2(ah[j]);
-        qf[c * 8 + 2 * j] = f.x * p.scale;
-        qf[c * 8 + 2 * j + 1] = f.y * p.scale;
-        kh[c * 4 + j] = bh[j];
-        vh[c * 4 + j] = ch[j];
-      }
-    }
-  }
-  // rotary on dims [0, 32): interleaved pairs (x0, x1) -> (x0 c - x1 s, x1 c + x0 s)
-  if (part * DP < 32 && act) {
-#pragma unroll
-    for (int j = 0; j < HP; ++j) {
-      const int pair = part * HP + j;
-      if (pair < 16) {
-        const float c = p.rot[(i * 16 + pair) * 2], s = p.rot[(i * 16 + pair) * 2 + 1];
-        const float q0 = qf[2 * j], q1 = qf[2 * j + 1];
-        qf[2 * j] = q0 * c - q1 * s;
-        qf[2 * j + 1] = q1 * c + q0 * s;
-        const float2 kf = __half22float2(kh[j]);
-        kh[j] = __floats2half2_rn(kf.x * c - kf.y * s, kf.y * c + kf.x * s);
-      }
-    }
-  }
-  // scores s[j] = q_i . k_j
-  float sc[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    float acc = 0.f;
-    if (j < p.F) {
-#pragma unroll
-      for (int d = 0; d < HP; ++d) {
-        uint32_t w = *reinterpret_cast<uint32_t*>(&kh[d]);
-        w = __shfl_sync(0xffffffff, w, j * 4 + part);
-        const float2 kf = __half22float2(*reinterpret_cast<__half2*>(&w));
-        acc += qf[2 * d] * kf.x + qf[2 * d + 1] * kf.y;
-      }
-      acc += __shfl_xor_sync(0xffffffff, acc, 1);
-      acc += __shfl_xor_sync(0xffffffff, acc, 2);
-      acc += act ? p.bias[(h * p.F + i) * p.F + j] : 0.f;
-    } else {
-      acc = -INFINITY;
-    }
-    sc[j] = acc;
-  }
-  float mx = sc[0];
-#pragma unroll
-  for (int j = 1; j < 8; ++j) mx = fmaxf(mx, sc[j]);
-  float den = 0.f;
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    sc[j] = __expf(sc[j] - mx);
-    den += sc[j];
-  }
-  const float inv = 1.f / den;
-  float of[DP];
-#pragma unroll
-  for (int d = 0; d < DP; ++d) of[d] = 0.f;
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    if (j < p.F) {
-      const float pj = sc[j] * inv;
-#pragma unroll
-      for (int d = 0; d < HP; ++d) {
-        uint32_t w = *reinterpret_cast<uint32_t*>(&vh[d]);
-        w = __shfl_sync(0xffffffff, w, j * 4 + part);
-        const float2 vf = __half22float2(*reinterpret_cast<__half2*>(&w));
-        of[2 * d] += pj * vf.x;
-        of[2 * d + 1] += pj * vf.y;
-      }
-    }
-  }
-  if (act) {
-    __half* op = p.o + tok * p.ldo + off;
-#pragma unroll
-    for (int c = 0; c < DP / 8; ++c) {
-      uint4 o;
-      uint32_t* ow = reinterpret_cast<uint32_t*>(&o);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        __half2 r = __floats2half2_rn(of[c * 8 + 2 * j], of[c * 8 + 2 * j + 1]);
-        ow[j] = *reinterpret_cast<uint32_t*>(&r);
-      }
-      stg16(op + c * 8, o);
-    }
-  }
-}
-
 // ---------------------------------------------------------------------------------------
-// temporal attention on mma.sync: one warp per PAIR of heads of one (batch, pixel).
+// temporal attention for F <= 8 and an even head count, on mma.sync: one warp per PAIR of heads of one (batch, pixel).
 // The two items' 8 frames are stacked into one 16-row tile, so that
 //   S  = [Q_a; Q_b] K_a^T , [Q_a; Q_b] K_b^T   (two m16n8k16 n-blocks per k-step; the cross terms are discarded)
 //   O  = diag(P_a, P_b) [V_a; V_b]              (ONE k-step: the block-diagonal P is exactly the A fragment
 //                                                {P_a, 0, 0, P_b} built from the S accumulators in registers)
-// ~125 instructions per (pixel, head) instead of ~700 for the shuffle formulation above (which is kept for an odd
-// head count): the kernel becomes a pure 8 B/element stream.  Rotary (first 32 dims, interleaved pairs) is applied to
-// the 16-byte chunks on their way into shared memory; scale and the relative-position bias are applied to the fp32
+// ~125 instructions per (pixel, head) instead of ~700 for a warp-shuffle formulation with one lane per (frame, quarter
+// of the head dim): the kernel becomes a pure 8 B/element stream.  Rotary (first 32 dims, interleaved pairs) is applied
+// to the 16-byte chunks on their way into shared memory; scale and the relative-position bias are applied to the fp32
 // scores.
 // ---------------------------------------------------------------------------------------
 template <int D>
@@ -633,33 +445,22 @@ __global__ void __launch_bounds__(128)
   __syncwarp();
 
   const int g = lane >> 2, t4 = lane & 3;
-  // ---- S = Q K^T ----
-  float s0[4] = {0.f, 0.f, 0.f, 0.f}, s1[4] = {0.f, 0.f, 0.f, 0.f};
-  {
-    const int arow = (lane & 7) + ((lane >> 3) & 1) * 8, achk = lane >> 4;
-    const int brow = (lane & 7) + (lane >> 4) * 8, bchk = (lane >> 3) & 1;
-#pragma unroll
-    for (int kk = 0; kk < D / 16; ++kk) {
-      uint32_t a[4], bfr[4];
-      ldmatrix_x4(a, tile_ptr<D>(sQ, arow, kk * 2 + achk));
-      ldmatrix_x4(bfr, tile_ptr<D>(sK, brow, kk * 2 + bchk));
-      mma16816(s0, a, bfr[0], bfr[1]);  // keys of item a
-      mma16816(s1, a, bfr[2], bfr[3]);  // keys of item b
-    }
-  }
-  // ---- softmax over the <= 8 keys of each item: row g of item a lives in s0[0..1], row g of item b in s1[2..3] ----
+  // ---- S = Q K^T: the two n-blocks are the keys of item a (s[0]) and of item b (s[1]) ----
+  float s[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+  warp_qk<D, 1>(s, sQ, (lane & 7) + ((lane >> 3) & 1) * 8, sK, lane);
+  // ---- softmax over the <= 8 keys of each item: row g of item a lives in s[0][0..1], row g of item b in s[1][2..3] ----
   uint32_t pa, pb;
   {
     const int j0 = 2 * t4, j1 = j0 + 1;
     const bool row_ok = g < p.F;
     float xa0 = -INFINITY, xa1 = -INFINITY, xb0 = -INFINITY, xb1 = -INFINITY;
     if (row_ok && j0 < p.F) {
-      xa0 = s0[0] * p.scale + __ldg(p.bias + (h0 * p.F + g) * p.F + j0);
-      xb0 = s1[2] * p.scale + __ldg(p.bias + ((h0 + 1) * p.F + g) * p.F + j0);
+      xa0 = s[0][0] * p.scale + __ldg(p.bias + (h0 * p.F + g) * p.F + j0);
+      xb0 = s[1][2] * p.scale + __ldg(p.bias + ((h0 + 1) * p.F + g) * p.F + j0);
     }
     if (row_ok && j1 < p.F) {
-      xa1 = s0[1] * p.scale + __ldg(p.bias + (h0 * p.F + g) * p.F + j1);
-      xb1 = s1[3] * p.scale + __ldg(p.bias + ((h0 + 1) * p.F + g) * p.F + j1);
+      xa1 = s[0][1] * p.scale + __ldg(p.bias + (h0 * p.F + g) * p.F + j1);
+      xb1 = s[1][3] * p.scale + __ldg(p.bias + ((h0 + 1) * p.F + g) * p.F + j1);
     }
     float ma = fmaxf(xa0, xa1), mb = fmaxf(xb0, xb1);
     ma = fmaxf(ma, __shfl_xor_sync(0xffffffffu, ma, 1));
@@ -674,26 +475,16 @@ __global__ void __launch_bounds__(128)
     da += __shfl_xor_sync(0xffffffffu, da, 2);
     db += __shfl_xor_sync(0xffffffffu, db, 2);
     const float ia = da > 0.f ? 1.f / da : 0.f, ib = db > 0.f ? 1.f / db : 0.f;
-    __half2 ha = __floats2half2_rn(ea0 * ia, ea1 * ia), hb = __floats2half2_rn(eb0 * ib, eb1 * ib);
-    pa = *reinterpret_cast<uint32_t*>(&ha);
-    pb = *reinterpret_cast<uint32_t*>(&hb);
+    pa = pack_half2_rn(ea0 * ia, ea1 * ia);
+    pb = pack_half2_rn(eb0 * ib, eb1 * ib);
   }
   // ---- O = diag(P_a, P_b) [V_a; V_b] ----
   float o[D / 8][4];
 #pragma unroll
   for (int i = 0; i < D / 8; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
-  {
-    const uint32_t a[4] = {pa, 0u, 0u, pb};
-    const int vrow = (lane & 7) + ((lane >> 3) & 1) * 8;
-#pragma unroll
-    for (int nb = 0; nb < D / 16; ++nb) {
-      uint32_t bfr[4];
-      ldmatrix_x4_trans(bfr, tile_ptr<D>(sV, vrow, nb * 2 + (lane >> 4)));
-      mma16816(o[nb * 2], a, bfr[0], bfr[1]);
-      mma16816(o[nb * 2 + 1], a, bfr[2], bfr[3]);
-    }
-  }
-  // ---- O -> smem (Q tile) -> 16-byte stores ----
+  const uint32_t a[4] = {pa, 0u, 0u, pb};
+  warp_pv<D>(o, a, sV, 0, lane);
+  // ---- O (P is normalised) -> smem (Q tile) -> 16-byte stores ----
   __syncwarp();
 #pragma unroll
   for (int n = 0; n < D / 8; ++n) {
@@ -714,7 +505,7 @@ __global__ void __launch_bounds__(128)
 }
 
 // ---------------------------------------------------------------------------------------
-// temporal attention for F > 8 frames (clips longer than the pipeline's 8-frame windows): one warp per
+// temporal attention for any F and head count (all but the even-head F <= 8 windows of the pipeline): one warp per
 // (batch, pixel, head).  Queries are taken in 16-frame tiles; keys and values stream through per-warp
 // shared memory in 16-frame tiles and the softmax is online (running fp32 row max and sum, O
 // rescaled), so F has no upper bound.  Rotary is applied in fp32 while the mma fragments of dims
@@ -769,9 +560,7 @@ __global__ void __launch_bounds__(128)
   };
 
   const int g = lane >> 2, t4 = lane & 3;
-  const int arow = (lane & 7) + ((lane >> 3) & 1) * 8, achk = lane >> 4;
-  const int brow = (lane & 7) + (lane >> 4) * 8, bchk = (lane >> 3) & 1;
-  const int vrow = (lane & 7) + ((lane >> 3) & 1) * 8;
+  const int arow = (lane & 7) + ((lane >> 3) & 1) * 8;
 #pragma unroll 1
   for (int64_t q0 = 0; q0 < F; q0 += 16) {
     __syncwarp();  // the previous tile's output rows have left sQ
@@ -816,14 +605,7 @@ __global__ void __launch_bounds__(128)
           mma16816(s[nb], ql[kk], kh[0], kh[1]);
         }
       }
-#pragma unroll
-      for (int kk = 2; kk < D / 16; ++kk) {
-        uint32_t qa[4], bfr[4];
-        ldmatrix_x4(qa, tile_ptr<D>(sQ, arow, kk * 2 + achk));
-        ldmatrix_x4(bfr, tile_ptr<D>(sK, brow, kk * 2 + bchk));
-        mma16816(s[0], qa, bfr[0], bfr[1]);
-        mma16816(s[1], qa, bfr[2], bfr[3]);
-      }
+      warp_qk<D, 1, 2>(s, sQ, arow, sK, lane);  // dims [32, D)
       float mx0 = -INFINITY, mx1 = -INFINITY;
 #pragma unroll
       for (int nb = 0; nb < 2; ++nb) {
@@ -872,21 +654,9 @@ __global__ void __launch_bounds__(128)
       }
       // ---- O += P V: the S accumulators are the A fragment of the k = 16 keys step ----
       uint32_t a[4];
-      {
-        __half2 h0 = __floats2half2_rn(s[0][0], s[0][1]), h1 = __floats2half2_rn(s[0][2], s[0][3]);
-        __half2 h2 = __floats2half2_rn(s[1][0], s[1][1]), h3 = __floats2half2_rn(s[1][2], s[1][3]);
-        a[0] = *reinterpret_cast<uint32_t*>(&h0);
-        a[1] = *reinterpret_cast<uint32_t*>(&h1);
-        a[2] = *reinterpret_cast<uint32_t*>(&h2);
-        a[3] = *reinterpret_cast<uint32_t*>(&h3);
-      }
-#pragma unroll
-      for (int nb = 0; nb < D / 16; ++nb) {
-        uint32_t bfr[4];
-        ldmatrix_x4_trans(bfr, tile_ptr<D>(sV, vrow, nb * 2 + (lane >> 4)));
-        mma16816(o[nb * 2], a, bfr[0], bfr[1]);
-        mma16816(o[nb * 2 + 1], a, bfr[2], bfr[3]);
-      }
+      pack_p(a, 0, s[0][0], s[0][1], s[0][2], s[0][3]);
+      pack_p(a, 1, s[1][0], s[1][1], s[1][2], s[1][3]);
+      warp_pv<D>(o, a, sV, 0, lane);
     }
     l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
     l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
@@ -895,11 +665,7 @@ __global__ void __launch_bounds__(128)
     const float i0 = 1.f / l0, i1 = 1.f / l1;
     // ---- O -> smem (Q tile) -> 16-byte stores of the rows < F ----
     __syncwarp();
-#pragma unroll
-    for (int n = 0; n < D / 8; ++n) {
-      *reinterpret_cast<__half2*>(tile_ptr<D>(sQ, g, n) + 2 * t4) = __floats2half2_rn(o[n][0] * i0, o[n][1] * i0);
-      *reinterpret_cast<__half2*>(tile_ptr<D>(sQ, g + 8, n) + 2 * t4) = __floats2half2_rn(o[n][2] * i1, o[n][3] * i1);
-    }
+    stage_rows<D>(sQ, g, o, i0, i1, t4);
     __syncwarp();
 #pragma unroll
     for (int i = 0; i < LD_ITERS; ++i) {
@@ -918,16 +684,37 @@ uav_status_t attention_tc(const void* q, const void* k, const void* v, void* out
                           int64_t ldv, int64_t ldo, int64_t kv_batch_div, float scale,
                           cudaStream_t stream);  // attention_tc.cu (wgmma)
 
-static uav_status_t launch_fa(const FaParams& p, int batch, cudaStream_t stream) {
-  constexpr int smem = (FA_BM + 4 * FA_BN) * FA_D * 2;
-  const uav_status_t st = opt_in_smem<flash_attn_kernel>(smem);
+// the opt-in, launch and launch check of flash_attn_kernel and every cross_attn_kernel
+template <auto Kernel>
+static uav_status_t launch_fa(const FaParams& p, dim3 grid, int smem, cudaStream_t stream) {
+  const uav_status_t st = opt_in_smem<Kernel>(smem);
   if (st != UAV_OK) return st;
-  dim3 grid((p.nq + FA_BM - 1) / FA_BM, batch * p.heads);
-  flash_attn_kernel<<<grid, FA_THREADS, smem, stream>>>(p);
+  Kernel<<<grid, FA_THREADS, smem, stream>>>(p);
   UAV_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(1, std::memory_order_relaxed);
   return UAV_OK;
 }
+
+template <int D, int NB16>
+static uav_status_t launch_cross(const FaParams& p, int batch, cudaStream_t stream) {
+  const int ntiles = (p.nq + FA_BM - 1) / FA_BM;
+  // enough CTAs to fill the GPU ~4x over, each streaming several query tiles past its resident K/V
+  int gx = (num_sms() * 8 + batch * p.heads - 1) / (batch * p.heads);
+  if (gx > ntiles) gx = ntiles;
+  if (gx < 1) gx = 1;
+  return launch_fa<cross_attn_kernel<D, NB16>>(p, dim3(gx * p.heads, batch), (2 * NB16 * 16 * D + 2 * FA_BM * D) * 2,
+                                               stream);
+}
+
+// blocks of 4 warps, one warp per (batch, pixel) and pair of heads (pairs) or head
+template <int D>
+static void launch_temporal(const TaParams& p, bool pairs, unsigned blocks, cudaStream_t stream) {
+  if (pairs) temporal_attn_mma_kernel<D><<<blocks, 128, 0, stream>>>(p);
+  else temporal_attn_long_kernel<D><<<blocks, 128, 0, stream>>>(p);
+}
+
+static bool misaligned16(const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) != 0; }
+#define UAV_REQUIRE_ALIGNED16(fn, ptr) UAV_REQUIRE(!misaligned16(ptr), fn ": " #ptr " must be 16-byte aligned")
 
 }  // namespace uav
 
@@ -947,35 +734,35 @@ uav_status_t uav_attention(const void* q, const void* k, const void* v, void* ou
               "uav_attention: token strides must be multiples of 8");
   UAV_REQUIRE(batch * heads <= 65535, "uav_attention: batch*heads too large");
   UAV_REQUIRE(batch % kv_batch_div == 0, "uav_attention: batch must be a multiple of kv_batch_div");
-  if (nk <= 128 && nq >= 4 * nk && (head_dim == 64 || head_dim == 128)) {
-    // short key/value sequence (the 77 prompt tokens): resident-KV streaming kernel
-    FaParams pc;
-    pc.q = (const __half*)q; pc.k = (const __half*)k; pc.v = (const __half*)v; pc.o = (__half*)out;
-    pc.ldq = ldq; pc.ldk = ldk; pc.ldv = ldv; pc.ldo = ldo;
-    pc.bsq = nq * ldq; pc.bsk = nk * ldk; pc.bsv = nk * ldv; pc.bso = nq * ldo;
-    pc.nq = (int)nq; pc.nk = (int)nk; pc.heads = heads; pc.kv_batch_div = (int)kv_batch_div;
-    pc.scale_log2 = scale * 1.4426950408889634f;
-    if (head_dim == 64) return nk <= 80 ? launch_cross<64, 5>(pc, (int)batch, stream) : launch_cross<64, 8>(pc, (int)batch, stream);
-    return nk <= 80 ? launch_cross<128, 5>(pc, (int)batch, stream) : launch_cross<128, 8>(pc, (int)batch, stream);
+  if (head_dim != 64 && head_dim != 128 && head_dim != 512) {
+    set_last_error("uav_attention: head_dim %d unsupported (64, 128, 512)", head_dim);
+    return UAV_ERR_UNSUPPORTED;
   }
-  // d = 128 (UNet self-attention at h/8) and d = 512 (VAE AttentionBlock) run on the wgmma kernel
-  if (head_dim == 128 || head_dim == 512)
+  UAV_REQUIRE(head_dim != 512 || heads == 1, "uav_attention: head_dim 512 supports a single head");
+  UAV_REQUIRE(nq <= INT32_MAX && nk <= INT32_MAX, "uav_attention: nq or nk too large");
+  UAV_REQUIRE_ALIGNED16("uav_attention", q);
+  UAV_REQUIRE_ALIGNED16("uav_attention", k);
+  UAV_REQUIRE_ALIGNED16("uav_attention", v);
+  UAV_REQUIRE_ALIGNED16("uav_attention", out);
+
+  // short key/value sequences (the 77 prompt tokens) run on the resident-KV streaming kernel; otherwise d = 128 (UNet
+  // self-attention at h/8) and d = 512 (VAE AttentionBlock) run on the wgmma kernel and d = 64 on flash_attn_kernel
+  const bool cross = nk <= 128 && nq >= 4 * nk && head_dim != 512;
+  if (!cross && head_dim != 64)
     return attention_tc(q, k, v, out, batch, heads, head_dim, nq, nk, ldq, ldk, ldv, ldo, kv_batch_div, scale,
                         stream);
-  if (head_dim == 64) {
-    FaParams p;
-    p.q = (const __half*)q;
-    p.k = (const __half*)k;
-    p.v = (const __half*)v;
-    p.o = (__half*)out;
-    p.ldq = ldq; p.ldk = ldk; p.ldv = ldv; p.ldo = ldo;
-    p.bsq = nq * ldq; p.bsk = nk * ldk; p.bsv = nk * ldv; p.bso = nq * ldo;
-    p.nq = (int)nq; p.nk = (int)nk; p.heads = heads; p.kv_batch_div = (int)kv_batch_div;
-    p.scale_log2 = scale * 1.4426950408889634f;
-    return launch_fa(p, (int)batch, stream);
+  FaParams p;
+  p.q = (const __half*)q; p.k = (const __half*)k; p.v = (const __half*)v; p.o = (__half*)out;
+  p.ldq = ldq; p.ldk = ldk; p.ldv = ldv; p.ldo = ldo;
+  p.bsq = nq * ldq; p.bsk = nk * ldk; p.bsv = nk * ldv; p.bso = nq * ldo;
+  p.nq = (int)nq; p.nk = (int)nk; p.heads = heads; p.kv_batch_div = (int)kv_batch_div;
+  p.scale_log2 = scale * 1.4426950408889634f;
+  if (cross) {
+    if (head_dim == 64) return nk <= 80 ? launch_cross<64, 5>(p, (int)batch, stream) : launch_cross<64, 8>(p, (int)batch, stream);
+    return nk <= 80 ? launch_cross<128, 5>(p, (int)batch, stream) : launch_cross<128, 8>(p, (int)batch, stream);
   }
-  set_last_error("uav_attention: head_dim %d unsupported (64, 128, 512)", head_dim);
-  return UAV_ERR_UNSUPPORTED;
+  return launch_fa<flash_attn_kernel>(p, dim3((p.nq + FA_BM - 1) / FA_BM, batch * heads), (FA_BM + 4 * FA_BN) * FA_D * 2,
+                                      stream);
 }
 
 uav_status_t uav_temporal_attention(const void* q, const void* k, const void* v, void* out,
@@ -990,34 +777,26 @@ uav_status_t uav_temporal_attention(const void* q, const void* k, const void* v,
   UAV_REQUIRE(B <= INT32_MAX && F <= INT32_MAX, "uav_temporal_attention: B or F too large");
   UAV_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0,
               "uav_temporal_attention: token strides must be multiples of 8");
+  if (head_dim != 64 && head_dim != 128) {
+    set_last_error("uav_temporal_attention: head_dim %d unsupported (64, 128)", head_dim);
+    return UAV_ERR_UNSUPPORTED;
+  }
+  UAV_REQUIRE_ALIGNED16("uav_temporal_attention", q);
+  UAV_REQUIRE_ALIGNED16("uav_temporal_attention", k);
+  UAV_REQUIRE_ALIGNED16("uav_temporal_attention", v);
+  UAV_REQUIRE_ALIGNED16("uav_temporal_attention", out);
+  UAV_REQUIRE_ALIGNED16("uav_temporal_attention", rot_cos_sin);
+  // the pipeline's windows (F <= 8, even head count): one warp per pair of heads; everything else: one warp per head
+  const bool pairs = F <= 8 && heads % 2 == 0;
+  const int64_t blocks = (B * HW * (pairs ? heads / 2 : heads) + 3) / 4;  // 4 warps per CTA
+  UAV_REQUIRE(blocks <= INT32_MAX, "uav_temporal_attention: too many (pixel, head) items");
   TaParams p;
   p.q = (const __half*)q; p.k = (const __half*)k; p.v = (const __half*)v; p.o = (__half*)out;
   p.ldq = ldq; p.ldk = ldk; p.ldv = ldv; p.ldo = ldo;
   p.B = (int)B; p.F = (int)F; p.heads = heads; p.HW = HW;
   p.scale = scale; p.rot = rot_cos_sin; p.bias = rel_bias;
-  const int64_t warps = B * HW * heads;
-  const unsigned grid = (unsigned)((warps + 7) / 8);
-  if (F > 8) {
-    // longer than the pipeline's windows: online softmax over 16-frame key tiles, one warp per (pixel, head)
-    UAV_REQUIRE((warps + 3) / 4 <= INT32_MAX, "uav_temporal_attention: too many (pixel, head) items");
-    const unsigned grid4 = (unsigned)((warps + 3) / 4);
-    if (head_dim == 64) temporal_attn_long_kernel<64><<<grid4, 128, 0, stream>>>(p);
-    else if (head_dim == 128) temporal_attn_long_kernel<128><<<grid4, 128, 0, stream>>>(p);
-    else {
-      set_last_error("uav_temporal_attention: head_dim %d unsupported (64, 128)", head_dim);
-      return UAV_ERR_UNSUPPORTED;
-    }
-  } else if (heads % 2 == 0 && (head_dim == 64 || head_dim == 128)) {
-    // mma.sync formulation: one warp per pair of heads
-    const unsigned grid2 = (unsigned)((warps / 2 + 3) / 4);
-    if (head_dim == 64) temporal_attn_mma_kernel<64><<<grid2, 128, 0, stream>>>(p);
-    else temporal_attn_mma_kernel<128><<<grid2, 128, 0, stream>>>(p);
-  } else if (head_dim == 64) temporal_attn_kernel<64><<<grid, 256, 0, stream>>>(p);
-  else if (head_dim == 128) temporal_attn_kernel<128><<<grid, 256, 0, stream>>>(p);
-  else {
-    set_last_error("uav_temporal_attention: head_dim %d unsupported (64, 128)", head_dim);
-    return UAV_ERR_UNSUPPORTED;
-  }
+  if (head_dim == 64) launch_temporal<64>(p, pairs, (unsigned)blocks, stream);
+  else launch_temporal<128>(p, pairs, (unsigned)blocks, stream);
   UAV_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(1, std::memory_order_relaxed);
   return UAV_OK;

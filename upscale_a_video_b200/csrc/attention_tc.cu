@@ -48,11 +48,6 @@ struct FaTcCfg {
   static constexpr int SMEM_BYTES = Q_BYTES + STAGES * SLOT_BYTES + 1024 + 1024;
 };
 
-__device__ __forceinline__ uint32_t pack_half2_rn(float a, float b) {
-  __half2 h = __floats2half2_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&h);
-}
-
 template <int DQK, int DVT, int BN>
 __global__ void __launch_bounds__(TC_THREADS, 1)
     fa_tc_kernel(const __grid_constant__ FaTcParams p) {
@@ -252,14 +247,11 @@ static uav_status_t launch_fa_tc(FaTcParams& p, int64_t batch, int dv_splits, cu
 }
 
 
-// entry used by uav_attention (attention.cu) for head_dim 128 and 512
+// entry used by uav_attention (attention.cu), which has validated the arguments, for head_dim 128 and 512 (one head)
 uav_status_t attention_tc(const void* q, const void* k, const void* v, void* out, int64_t batch,
                           int heads, int head_dim, int64_t nq, int64_t nk, int64_t ldq, int64_t ldk,
                           int64_t ldv, int64_t ldo, int64_t kv_batch_div, float scale,
                           cudaStream_t stream) {
-  UAV_REQUIRE((reinterpret_cast<uintptr_t>(q) & 15) == 0 && (reinterpret_cast<uintptr_t>(k) & 15) == 0 &&
-                  (reinterpret_cast<uintptr_t>(v) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0,
-              "attention_tc: pointers must be 16-byte aligned");
   FaTcParams p;
   memset(&p, 0, sizeof(p));
   const int64_t C = (int64_t)heads * head_dim;
@@ -285,13 +277,8 @@ uav_status_t attention_tc(const void* q, const void* k, const void* v, void* out
   p.heads = heads;
   p.kv_batch_div = (int)kv_batch_div;
   p.scale_log2 = scale * 1.4426950408889634f;
-  if (head_dim == 512) {
-    UAV_REQUIRE(heads == 1, "attention_tc: head_dim 512 supports a single head");
-    return launch_fa_tc<512, 256, 64>(p, batch, 2, stream);
-  }
-  if (head_dim == 128) return launch_fa_tc<128, 128, 128>(p, batch, 1, stream);
-  set_last_error("attention_tc: head_dim %d unsupported", head_dim);
-  return UAV_ERR_UNSUPPORTED;
+  if (head_dim == 512) return launch_fa_tc<512, 256, 64>(p, batch, 2, stream);
+  return launch_fa_tc<128, 128, 128>(p, batch, 1, stream);
 }
 
 }  // namespace uav

@@ -63,18 +63,6 @@ __device__ __forceinline__ float mul16(float a, float b) { return rh16(__fmul_rn
 __device__ __forceinline__ float add16(float a, float b) { return rh16(__fadd_rn(a, b)); }
 __device__ __forceinline__ float sub16(float a, float b) { return rh16(__fsub_rn(a, b)); }
 
-__device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], const void* p) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-               : "r"(smem_u32(p)));
-}
-__device__ __forceinline__ void mma_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
 __global__ void __launch_bounds__(CO_THREADS, 1)
     conv_out_fused_kernel(const ConvOutParams p) {
   extern __shared__ __align__(128) uint8_t co_smem[];
@@ -173,18 +161,18 @@ __global__ void __launch_bounds__(CO_THREADS, 1)
         for (int m = 0; m < 2; ++m) {
           const int row = warp * 32 + m * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
           const int chk = ks * 2 + (lane >> 4);
-          ldsm_x4(a[m], xb + row * CO_KC + ((chk ^ (row & 7)) << 3));
+          ldmatrix_x4(a[m], xb + row * CO_KC + ((chk ^ (row & 7)) << 3));
         }
 #pragma unroll
         for (int nb = 0; nb < 3; ++nb) {
           uint32_t bf[4];
           const int row = nb * 16 + (lane & 7) + (lane >> 4) * 8;
           const int chk = kc * 8 + ks * 2 + ((lane >> 3) & 1);
-          ldsm_x4(bf, ws + row * CO_C + ((chk ^ (row & 7)) << 3));
+          ldmatrix_x4(bf, ws + row * CO_C + ((chk ^ (row & 7)) << 3));
 #pragma unroll
           for (int m = 0; m < 2; ++m) {
-            mma_16816(acc[m][nb * 2], a[m], bf[0], bf[1]);
-            mma_16816(acc[m][nb * 2 + 1], a[m], bf[2], bf[3]);
+            mma16816(acc[m][nb * 2], a[m], bf[0], bf[1]);
+            mma16816(acc[m][nb * 2 + 1], a[m], bf[2], bf[3]);
           }
         }
       }

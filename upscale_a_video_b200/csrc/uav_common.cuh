@@ -260,6 +260,53 @@ __device__ __forceinline__ void stg16(void* p, const uint4& v) {
   *reinterpret_cast<uint4*>(p) = v;
 }
 
+// fp32 pair -> packed fp16, round to nearest
+__device__ __forceinline__ uint32_t pack_half2_rn(float a, float b) {
+  __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&h);
+}
+
+// ---- cp.async / ldmatrix / mma.sync m16n8k16 (warp-level MMA) ----
+__device__ __forceinline__ void cp_async16(void* smem, const void* gmem, bool valid) {
+  const uint32_t s = smem_u32(smem);
+  const int sz = valid ? 16 : 0;
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(s), "l"(gmem), "r"(sz)
+               : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() {
+  asm volatile("cp.async.commit_group;" ::: "memory");
+}
+template <int N>
+__device__ __forceinline__ void cp_async_wait() {
+  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
+}
+__device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], const void* p) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(smem_u32(p)));
+}
+__device__ __forceinline__ void ldmatrix_x4_trans(uint32_t (&r)[4], const void* p) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(smem_u32(p)));
+}
+// c += a b: a is the 16 x 16 A fragment, (b0, b1) the 16 x 8 B fragment, c the fp32 16 x 8 accumulator (c[0..1] row
+// lane / 4, c[2..3] row lane / 4 + 8, columns 2 (lane % 4) + {0, 1})
+__device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0,
+                                         uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, "
+      "{%0,%1,%2,%3};"
+      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
+// smem tile: rows of DT halfs, 16-byte chunks XOR-swizzled by (row & 7)
+template <int DT>
+__device__ __forceinline__ __half* tile_ptr(__half* base, int row, int chunk) {
+  return base + row * DT + ((chunk ^ (row & 7)) << 3);
+}
+
 // ---------------------------------------------------------------------------------------
 // launch plumbing (host)
 // ---------------------------------------------------------------------------------------
