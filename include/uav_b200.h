@@ -356,6 +356,20 @@ uav_status_t uav_wavelet_level(const float* image, int64_t planes, int64_t H, in
  * frames: [T][C][H][W] fp32, out: [T][H][W][C] uint8, C <= 4. Bit-exact. */
 uav_status_t uav_pack_video_uint8(const float* frames, int64_t T, int64_t C, int64_t H, int64_t W, uint8_t* out,
                                   uav_stream_t stream);
+/* the PNG rounding of torchvision save_image(normalize=True, value_range=(-1, 1)) (inference_upscale_a_video.py:350):
+ * clamp(-1, 1), (x + 1) / 2, * 255, + 0.5, clamp(0, 255), truncate. Same layout as uav_pack_video_uint8. Bit-exact. */
+uav_status_t uav_pack_frames_png(const float* frames, int64_t T, int64_t C, int64_t H, int64_t W, uint8_t* out,
+                                 uav_stream_t stream);
+
+/* ---- before sampling: frame ingest (inference_upscale_a_video.py:180-188) ------------------------------------
+ * frames: [T][H][W][3] uint8 in BGR order (OpenCV's decode); out: [3][T][h_out][w_out] fp32 RGB in [-1, 1]:
+ * (v / 255. - 0.5) * 2 with one IEEE fp32 rounding per op, then, when (h_out, w_out) != (H, W),
+ * F.interpolate(x, (h_out, w_out), mode='area') bit-identical to torch's CUDA kernel for NCHW fp32 frames (nhwc = 0:
+ * the reference's image folders, made contiguous by utils.read_frame_from_videos) or for channels-last ones (nhwc = 1:
+ * its video files, which torchvision.io.read_video returns as a permuted view). The two kernels round the average
+ * differently. 1 <= h_out <= H, 1 <= w_out <= W, not a 1x1 output of a larger frame. */
+uav_status_t uav_unpack_video_uint8(const uint8_t* frames, int64_t T, int64_t H, int64_t W, int64_t h_out, int64_t w_out,
+                                    int nhwc, float* out, uav_stream_t stream);
 
 /* ---- RAFT bidirectional optical flow (SURVEY.md §8f rank 1; models_video/RAFT) -----------------------------
  * Non-GEMM kernels; activations channels-last fp16 [pixel][C], correlation volume / coordinates / flows fp32. */

@@ -103,6 +103,8 @@ _PROTOS = {
     "uav_adain_apply": [P, I64, I64, P, P, P, P, P, P],
     "uav_wavelet_level": [P, I64, I64, I64, I32, P, P, I32, P, P],
     "uav_pack_video_uint8": [P, I64, I64, I64, I64, P, P],
+    "uav_pack_frames_png": [P, I64, I64, I64, I64, P, P],
+    "uav_unpack_video_uint8": [P, I64, I64, I64, I64, I64, I32, P, P],
 }
 _SPECIAL = {
     "uav_version": (C.c_char_p, []),

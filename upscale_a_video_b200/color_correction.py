@@ -10,7 +10,8 @@ import torch
 from . import _lib, ops
 
 __all__ = ["calc_mean_std", "adaptive_instance_normalization", "adain_color_fix", "wavelet_blur", "wavelet_decomposition",
-           "wavelet_reconstruction", "wavelet_color_fix", "upsample_lr_frames", "color_fix_frames", "pack_video_uint8"]
+           "wavelet_reconstruction", "wavelet_color_fix", "upsample_lr_frames", "color_fix_frames", "pack_video_uint8",
+           "pack_frames_png"]
 
 
 def _check(x: torch.Tensor, name: str):
@@ -105,3 +106,10 @@ def color_fix_frames(output: torch.Tensor, vframes: torch.Tensor, color_fix: Opt
 def pack_video_uint8(frames: torch.Tensor) -> torch.Tensor:
     """inference_upscale_a_video.py:354-356: (t, c, h, w) in [-1, 1] -> (t, h, w, c) uint8 on the device"""
     return ops.pack_video_uint8(frames)
+
+
+def pack_frames_png(frames: torch.Tensor) -> torch.Tensor:
+    """inference_upscale_a_video.py:350 (save_image(normalize=True, value_range=(-1, 1))): (t, c, h, w) -> (t, h, w, c)
+    uint8 on the device"""
+    _lib.require_cuda(frames, "pack_frames_png")
+    return ops.pack_frames_png(frames)

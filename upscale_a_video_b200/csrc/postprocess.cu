@@ -1,6 +1,7 @@
 // postprocess.cu — the step right after the decode (SURVEY.md §8f rank 4): bicubic x4 of the low-resolution
-// frames, AdaIN / wavelet colour fix against them, and the uint8 THWC packing of the result
-// (inference_upscale_a_video.py:323-357, models_video/color_correction.py:45-118).
+// frames, AdaIN / wavelet colour fix against them, and the uint8 THWC packing of the result for the mp4 and the PNG
+// frames (inference_upscale_a_video.py:323-357, models_video/color_correction.py:45-118); and the frame ingest before
+// sampling (uint8 frames -> normalised, area-resized fp32 clip, inference_upscale_a_video.py:180-188).
 //
 // All tensors are the reference's own planar fp32 "t c h w" frames.  Every kernel is a single streaming pass
 // (HBM-bound: the 4x frames are the largest tensors of the whole job, 283 MB per 8-frame 1280x2304 clip):
@@ -175,8 +176,12 @@ __global__ void wavelet_level_kernel(const float* __restrict__ img, int64_t plan
 }
 
 // ---------------------------------------------------------------------------------------
-// (x / 2 + 0.5).clamp(0, 1) * 255 -> "t h w c" -> uint8 (truncation, as numpy astype)   (inference…:354-356)
+// "t c h w" fp32 -> "t h w c" uint8 by truncation, with one of two roundings:
+//   video (inference…:354-356):  (x / 2 + 0.5).clamp(0, 1) * 255, then numpy astype
+//   PNG   (torchvision save_image(normalize=True, value_range=(-1, 1)), inference…:350):
+//         clamp(-1, 1), (x - (-1)) / 2, * 255, + 0.5, clamp(0, 255), then Tensor.to(uint8)
 // ---------------------------------------------------------------------------------------
+template <bool PNG>
 __global__ void pack_uint8_kernel(const float* __restrict__ x, int64_t T, int C, int64_t hw, uint8_t* __restrict__ out) {
   const int64_t total = T * hw;
   UAV_PP_GRID_STRIDE(i, total) {
@@ -184,11 +189,59 @@ __global__ void pack_uint8_kernel(const float* __restrict__ x, int64_t T, int C,
     const float* src = x + t * C * hw + px;
     uint8_t* dst = out + i * C;
     for (int c = 0; c < C; ++c) {
-      float v = __fadd_rn(__fmul_rn(src[c * hw], 0.5f), 0.5f);  // x / 2 is exact either way
-      v = fminf(fmaxf(v, 0.f), 1.f);
-      v = __fmul_rn(v, 255.f);
+      float v;
+      if (PNG) {
+        v = fminf(fmaxf(src[c * hw], -1.f), 1.f);
+        v = __fmul_rn(__fadd_rn(v, 1.f), 0.5f);  // the halving is exact, as is the reference's division by 2
+        v = __fadd_rn(__fmul_rn(v, 255.f), 0.5f);
+        v = fminf(fmaxf(v, 0.f), 255.f);
+      } else {
+        v = __fadd_rn(__fmul_rn(src[c * hw], 0.5f), 0.5f);  // x / 2 is exact either way
+        v = fminf(fmaxf(v, 0.f), 1.f);
+        v = __fmul_rn(v, 255.f);
+      }
       dst[c] = static_cast<uint8_t>(static_cast<int>(v));  // NaN -> 0 (numpy gives an unspecified value)
     }
+  }
+}
+
+// ---------------------------------------------------------------------------------------
+// frame ingest (inference…:180-188): uint8 "t h w c" BGR frames (OpenCV's decode order) -> planar fp32 RGB "c t h w".
+//   * normalisation (v / 255. - 0.5) * 2 with the three roundings of the reference's CPU ops (an IEEE division, not
+//     the reciprocal multiply torch uses for a scalar divisor on the GPU);
+//   * area resize to (h_out, w_out) in the same pass, as ATen's adaptive_avg_pool2d CUDA kernels: fp32 sum over the
+//     window in (row, column) order from 0, then, for NCHW frames, two divisions sum / kh / kw, and for channels-last
+//     frames (NHWC) one multiply by the fp32 reciprocal 1 / (kh * kw).  The two differ once kh * kw is not a power of
+//     two, i.e. for overlapping windows (and both differ from the single divide of the 3-D kernel behind
+//     uav_flow_resize_area).  A 1 x 1 window (no resize) returns the normalised value unchanged.
+// One thread per output pixel reads the 3 bytes of each input pixel of its window.
+// ---------------------------------------------------------------------------------------
+__device__ __forceinline__ float normalize_u8(uint8_t u) {
+  return __fmul_rn(__fsub_rn(__fdiv_rn(static_cast<float>(u), 255.f), 0.5f), 2.f);
+}
+
+template <bool NHWC>
+__global__ void unpack_uint8_kernel(const uint8_t* __restrict__ in, int64_t T, int64_t H, int64_t W, int64_t h_out,
+                                    int64_t w_out, float* __restrict__ out) {
+  const int64_t hw_out = h_out * w_out;
+  const int64_t total = T * hw_out;
+  UAV_PP_GRID_STRIDE(i, total) {
+    const int64_t ox = i % w_out, oy = (i / w_out) % h_out, t = i / hw_out;
+    const int64_t y0 = area_start(oy, h_out, H), y1 = area_end(oy, h_out, H);
+    const int64_t x0 = area_start(ox, w_out, W), x1 = area_end(ox, w_out, W);
+    float sum[3] = {0.f, 0.f, 0.f};
+    for (int64_t y = y0; y < y1; ++y) {
+      const uint8_t* row = in + (t * H + y) * W * 3;
+      for (int64_t x = x0; x < x1; ++x) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) sum[c] = __fadd_rn(sum[c], normalize_u8(__ldg(row + x * 3 + c)));
+      }
+    }
+    const float kh = static_cast<float>(y1 - y0), kw = static_cast<float>(x1 - x0);
+    const float factor = __fdiv_rn(1.f, static_cast<float>((y1 - y0) * (x1 - x0)));
+#pragma unroll
+    for (int c = 0; c < 3; ++c)  // BGR -> RGB
+      out[(2 - c) * total + i] = NHWC ? __fmul_rn(sum[c], factor) : __fdiv_rn(__fdiv_rn(sum[c], kh), kw);
   }
 }
 
@@ -257,7 +310,35 @@ uav_status_t uav_wavelet_level(const float* image, int64_t planes, int64_t H, in
 uav_status_t uav_pack_video_uint8(const float* frames, int64_t T, int64_t C, int64_t H, int64_t W, uint8_t* out,
                                   uav_stream_t stream) {
   UAV_REQUIRE(frames && out && T > 0 && C > 0 && C <= 4 && H > 0 && W > 0, "uav_pack_video_uint8: bad argument");
-  pack_uint8_kernel<<<grid_for(T * H * W, 256), 256, 0, (cudaStream_t)stream>>>(frames, T, (int)C, H * W, out);
+  pack_uint8_kernel<false><<<grid_for(T * H * W, 256), 256, 0, (cudaStream_t)stream>>>(frames, T, (int)C, H * W, out);
+  UAV_CHECK_CUDA(cudaGetLastError());
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  return UAV_OK;
+}
+
+uav_status_t uav_pack_frames_png(const float* frames, int64_t T, int64_t C, int64_t H, int64_t W, uint8_t* out,
+                                 uav_stream_t stream) {
+  UAV_REQUIRE(frames && out && T > 0 && C > 0 && C <= 4 && H > 0 && W > 0, "uav_pack_frames_png: bad argument");
+  pack_uint8_kernel<true><<<grid_for(T * H * W, 256), 256, 0, (cudaStream_t)stream>>>(frames, T, (int)C, H * W, out);
+  UAV_CHECK_CUDA(cudaGetLastError());
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  return UAV_OK;
+}
+
+uav_status_t uav_unpack_video_uint8(const uint8_t* frames, int64_t T, int64_t H, int64_t W, int64_t h_out, int64_t w_out,
+                                    int nhwc, float* out, uav_stream_t stream) {
+  UAV_REQUIRE(frames && out && T > 0 && H > 0 && W > 0, "uav_unpack_video_uint8: bad argument");
+  UAV_REQUIRE(h_out > 0 && h_out <= H && w_out > 0 && w_out <= W,
+              "uav_unpack_video_uint8: output %lldx%lld must be between 1x1 and the input's %lldx%lld (downsampling only)",
+              (long long)h_out, (long long)w_out, (long long)H, (long long)W);
+  // torch reduces to a 1 x 1 output with a mean, whose summation order this kernel does not reproduce
+  UAV_REQUIRE(h_out > 1 || w_out > 1 || (H == 1 && W == 1), "uav_unpack_video_uint8: a 1x1 output is not supported");
+  UAV_REQUIRE(H < (1 << 30) && W < (1 << 30), "uav_unpack_video_uint8: frame too large");
+  const unsigned grid = grid_for(T * h_out * w_out, 256);
+  if (nhwc)
+    unpack_uint8_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>(frames, T, H, W, h_out, w_out, out);
+  else
+    unpack_uint8_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(frames, T, H, W, h_out, w_out, out);
   UAV_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(1, std::memory_order_relaxed);
   return UAV_OK;

@@ -240,15 +240,8 @@ __global__ void propagate_step_kernel(const void* feat_prop_, const void* feat_c
 // = adaptive_avg_pool3d: output (ot, oh, ow) averages the input window [floor(i*in/out),
 // ceil((i+1)*in/out)) in each dimension.  As torch's CUDA kernel: fp32 sum in (t, h, w) order,
 // one divide by the window size, rounded to the storage dtype; then `* scale` in fp32 opmath and
-// rounded again.  in/out are (planes, t, h, w) contiguous.
+// rounded again.  in/out are (planes, t, h, w) contiguous.  Window bounds: area_start / area_end (uav_common.cuh).
 // ---------------------------------------------------------------------------------------
-__device__ __forceinline__ int64_t area_start(int64_t o, int64_t out_size, int64_t in_size) {
-  return (o * in_size) / out_size;
-}
-__device__ __forceinline__ int64_t area_end(int64_t o, int64_t out_size, int64_t in_size) {
-  return ((o + 1) * in_size + out_size - 1) / out_size;
-}
-
 template <bool HALF>
 __global__ void flow_resize_area_kernel(const void* in_, void* out_, int64_t planes, int64_t t_in,
                                         int64_t h_in, int64_t w_in, int64_t t_out, int64_t h_out,

@@ -196,6 +196,16 @@ __device__ __forceinline__ void wgmma_rs_tb(float (&d)[32], const uint32_t (&a)[
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d));
 }
 
+// ---- adaptive average pooling (F.interpolate mode='area') ----
+// output index o of out_size averages the input window [floor(o * in / out), ceil((o + 1) * in / out)); windows of
+// neighbouring outputs overlap when in_size is not a multiple of out_size
+__device__ __forceinline__ int64_t area_start(int64_t o, int64_t out_size, int64_t in_size) {
+  return (o * in_size) / out_size;
+}
+__device__ __forceinline__ int64_t area_end(int64_t o, int64_t out_size, int64_t in_size) {
+  return ((o + 1) * in_size + out_size - 1) / out_size;
+}
+
 // ---- misc math ----
 // MUFU.EX2 / MUFU.RCP with flush-to-zero: the non-ftz forms (__expf, __fdividef) wrap every MUFU in denormal
 // range fix-ups (FSETP + predicated FMULs: ~8 extra instructions per GELU), which matters in the GEMM epilogues that

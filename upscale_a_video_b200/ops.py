@@ -746,6 +746,33 @@ def pack_video_uint8(frames: torch.Tensor) -> torch.Tensor:
     return out
 
 
+def pack_frames_png(frames: torch.Tensor) -> torch.Tensor:
+    """(t, c, h, w) -> (t, h, w, c) uint8 with the rounding of save_image(normalize=True, value_range=(-1, 1))"""
+    frames = _f32_planes(frames)
+    t, c, h, w = frames.shape
+    out = torch.empty(t, h, w, c, dtype=torch.uint8, device=frames.device)
+    lib = _lib.load()
+    _lib.check(lib.uav_pack_frames_png(frames.data_ptr(), t, c, h, w, out.data_ptr(), _stream()), "uav_pack_frames_png")
+    return out
+
+
+def unpack_video_uint8(frames: torch.Tensor, size=None, channels_last: bool = False) -> torch.Tensor:
+    """(t, h, w, 3) uint8 BGR frames on the GPU -> (1, 3, t, h_out, w_out) fp32 RGB in [-1, 1]; `size` = (h_out, w_out)
+    area-downsamples in the same pass (None: no resize), rounded as torch's area resize rounds NCHW frames, or
+    channels-last frames when `channels_last`"""
+    assert frames.is_cuda and frames.dtype == torch.uint8 and frames.dim() == 4 and frames.shape[-1] == 3, \
+        "expected CUDA (t, h, w, 3) uint8 frames"
+    frames = frames.contiguous()
+    t, h, w, _ = frames.shape
+    ho, wo = (h, w) if size is None else (int(s) for s in size)
+    out = torch.empty(1, 3, t, ho, wo, dtype=torch.float32, device=frames.device)
+    lib = _lib.load()
+    _lib.check(lib.uav_unpack_video_uint8(frames.data_ptr(), t, h, w, ho, wo, 1 if channels_last else 0, out.data_ptr(),
+                                          _stream()),
+               "uav_unpack_video_uint8")
+    return out
+
+
 # ---------------------------------------------------------------------------------------
 # RAFT optical flow (csrc/raft.cu + uav_conv2d_taps): channels-last fp16 activations, fp32 correlation / coordinates
 # ---------------------------------------------------------------------------------------
