@@ -178,6 +178,36 @@ def test_attention_validates_before_launch(uav_lib):
     assert uav_lib.uav_launch_count() == 0
 
 
+def test_streaming_kernels_validate_before_launch(uav_lib):
+    """the grid-stride entry points reject misaligned 16-byte operands, short row strides, unknown dtypes and sizes that
+    overflow the kernels' int indexing before anything launches.  The pointers are never dereferenced."""
+    A, M = 1 << 20, (1 << 20) + 8  # 16-byte aligned and misaligned fake pointers
+    L = uav_lib
+    launches = L.uav_launch_count()
+
+    def rejects(st, msg):
+        assert st == 1 and msg in L.uav_last_error_string(), (st, msg, L.uav_last_error_string())
+
+    rejects(L.uav_copy_channels(M, 64, A, 64, 64, 100, None), b"uav_copy_channels: src must be 16-byte aligned")
+    rejects(L.uav_copy_channels(A, 64, A, 64, 64, -1, None), b"uav_copy_channels: pixels must be >= 0")
+    rejects(L.uav_sft_fuse(A, A, A, 1.0, 1.0, M, 64, None), b"uav_sft_fuse: out must be 16-byte aligned")
+    rejects(L.uav_add_relu(A, M, A, 64, None), b"uav_add_relu: b must be 16-byte aligned")
+    rejects(L.uav_layernorm(A, 4, 64, 64, M, A, 1e-5, A, 64, None), b"uav_layernorm: gamma must be 16-byte aligned")
+    rejects(L.uav_instnorm_relu(A, 1, 16, 64, 1e-5, 1, M, A, None), b"uav_instnorm_relu: y must be 16-byte aligned")
+    rejects(L.uav_instnorm_relu(A, 65536, 16, 64, 1e-5, 1, A, A, None), b"uav_instnorm_relu: n must be at most 65535")
+    rejects(L.uav_upsample_nearest(A, 64, 1, 4, 4, 64, A, 32, 8, 8, None),
+            b"uav_upsample_nearest: ld_src and ld_dst must be >= C")
+    rejects(L.uav_upsample_nearest(A, 64, 1, 4, 4, 64, A, 64, 1 << 31, 8, None),
+            b"uav_upsample_nearest: Hi, Wi, Ho and Wo must be < 2^30")
+    rejects(L.uav_planar_to_channels_last(A, 7, 1, 3, 16, A, 8, 0, 1.0, None),
+            b"uav_planar_to_channels_last: unsupported src_dtype 7")
+    rejects(L.uav_raft_split_tanh_relu(A, 16, 128, A, 64, A, 384, None, 0, None), b"uav_raft_split_tanh_relu: ld_net")
+    rejects(L.uav_raft_gru_rh(A, 128, A, 384, A, 384, 16, 128, None), b"uav_raft_gru_rh: ld_zr must be >= 2C")
+    rejects(L.uav_raft_flow_update(A, None, 0, 16, 4, 4, A, 1, None, 0, None, 0, None), b"uav_raft_flow_update: ld_delta, ld16")
+    rejects(L.uav_raft_convex_upsample(A, A, 576, 1, 1 << 28, 4, A, None), b"uav_raft_convex_upsample: h8 and w8")
+    assert L.uav_launch_count() == launches
+
+
 def test_scheduler_host_tables_match_oracle():
     """DDIMScheduler's host-side schedule (timesteps, alphas) is plain CPU math: compare with the oracle without a GPU"""
     import json

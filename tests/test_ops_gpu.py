@@ -193,6 +193,11 @@ def test_cfg_blend_addnoise(dtype):
             ref[:, :, 3 + k] = src[:, :, k]
     ops.window_blend(dst, src, 3, 0b00011111)
     assert torch.equal(dst, ref)
+    from upscale_a_video_b200 import _lib
+    launches = _lib.launch_count()
+    with pytest.raises(AssertionError):  # a non-contiguous src is rejected before the kernel would read it as dense
+        ops.window_blend(dst, src.transpose(3, 4), 3, 0)
+    assert _lib.launch_count() == launches and torch.equal(dst, ref)
 
 
 @pytest.mark.parametrize("dtype", [torch.float16, torch.float32])

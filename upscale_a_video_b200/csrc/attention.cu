@@ -18,10 +18,7 @@
 // staging are written once.
 #include "uav_common.cuh"
 
-#include <atomic>
-
 namespace uav {
-extern std::atomic<uint64_t> g_launches;
 
 // ---------------------------------------------------------------------------------------
 // warp tiles: a warp owns 16 query rows.  Lane l holds rows l / 4 and l / 4 + 8 of every 16 x 8 accumulator block,
@@ -690,8 +687,7 @@ static uav_status_t launch_fa(const FaParams& p, dim3 grid, int smem, cudaStream
   const uav_status_t st = opt_in_smem<Kernel>(smem);
   if (st != UAV_OK) return st;
   Kernel<<<grid, FA_THREADS, smem, stream>>>(p);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
@@ -712,9 +708,6 @@ static void launch_temporal(const TaParams& p, bool pairs, unsigned blocks, cuda
   if (pairs) temporal_attn_mma_kernel<D><<<blocks, 128, 0, stream>>>(p);
   else temporal_attn_long_kernel<D><<<blocks, 128, 0, stream>>>(p);
 }
-
-static bool misaligned16(const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) != 0; }
-#define UAV_REQUIRE_ALIGNED16(fn, ptr) UAV_REQUIRE(!misaligned16(ptr), fn ": " #ptr " must be 16-byte aligned")
 
 }  // namespace uav
 
@@ -797,8 +790,7 @@ uav_status_t uav_temporal_attention(const void* q, const void* k, const void* v,
   p.scale = scale; p.rot = rot_cos_sin; p.bias = rel_bias;
   if (head_dim == 64) launch_temporal<64>(p, pairs, (unsigned)blocks, stream);
   else launch_temporal<128>(p, pairs, (unsigned)blocks, stream);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 

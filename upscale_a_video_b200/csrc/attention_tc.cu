@@ -18,11 +18,9 @@
 // operand of P V).
 #include "uav_common.cuh"
 
-#include <atomic>
 #include <string.h>
 
 namespace uav {
-extern std::atomic<uint64_t> g_launches;
 
 constexpr int TC_BM = 128;      // query rows per CTA (two warpgroups of 64)
 constexpr int TC_THREADS = 384;
@@ -241,8 +239,7 @@ static uav_status_t launch_fa_tc(FaTcParams& p, int64_t batch, int dv_splits, cu
   if (st != UAV_OK) return st;
   dim3 grid((p.nq + TC_BM - 1) / TC_BM, dv_splits, (unsigned)(batch * p.heads));
   fa_tc_kernel<DQK, DVT, BN><<<grid, TC_THREADS, Cfg::SMEM_BYTES, stream>>>(p);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 

@@ -3,12 +3,6 @@
 // CLIPTextModel): causal self-attention over the 77-token prompt.
 #include "uav_common.cuh"
 
-#include <atomic>
-
-namespace uav {
-extern std::atomic<uint64_t> g_launches;
-}
-
 // ---------------------------------------------------------------------------------------
 // CLIP text encoder (SURVEY.md §8f rank 3): causal self-attention over a short sequence (77 tokens) — the only attention
 // on the path that needs a mask.  One CTA per (batch, head): K and V of the head in shared memory, one warp per query row,
@@ -17,6 +11,11 @@ extern std::atomic<uint64_t> g_launches;
 // ---------------------------------------------------------------------------------------
 namespace uav {
 constexpr int CA_MAX_N = 128;
+
+// dynamic shared memory of a launch over n tokens of head_dim d
+constexpr size_t ca_smem_bytes(int64_t n, int64_t d) {
+  return n * (d + 2) * 2 + n * d * 2 + 4 * CA_MAX_N * sizeof(float) + 4 * d * sizeof(float);
+}
 
 __global__ void __launch_bounds__(128)
     causal_attn_kernel(const __half* __restrict__ q, const __half* __restrict__ k, const __half* __restrict__ v,
@@ -89,15 +88,13 @@ uav_status_t uav_attention_causal(const void* q, const void* k, const void* v, v
               "uav_attention_causal: sequence <= %d tokens and even head_dim <= 128 (got n=%lld d=%d)", uav::CA_MAX_N,
               (long long)n, head_dim);
   UAV_REQUIRE(batch <= 65535, "uav_attention_causal: batch too large");
-  const size_t smem = static_cast<size_t>(n) * (head_dim + 2) * 2 + static_cast<size_t>(n) * head_dim * 2 +
-                      4 * uav::CA_MAX_N * sizeof(float) + 4 * head_dim * sizeof(float);
-  if (smem > 48 * 1024)
-    UAV_CHECK_CUDA(cudaFuncSetAttribute(uav::causal_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const uav_status_t st = uav::opt_in_smem<uav::causal_attn_kernel>((int)uav::ca_smem_bytes(uav::CA_MAX_N, 128));
+  if (st != UAV_OK) return st;
+  const size_t smem = uav::ca_smem_bytes(n, head_dim);
   uav::causal_attn_kernel<<<dim3((unsigned)heads, (unsigned)batch), 128, smem, (cudaStream_t)stream>>>(
       reinterpret_cast<const __half*>(q), reinterpret_cast<const __half*>(k), reinterpret_cast<const __half*>(v),
       reinterpret_cast<__half*>(out), (int)n, head_dim, ldq, ldk, ldv, ldo, scale);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  uav::g_launches.fetch_add(1, std::memory_order_relaxed);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 

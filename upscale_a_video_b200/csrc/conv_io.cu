@@ -16,12 +16,9 @@
 // MMAs of the current one.
 #include "uav_common.cuh"
 
-#include <atomic>
 #include <string.h>
 
 namespace uav {
-extern std::atomic<uint64_t> g_launches;
-int num_sms();
 
 namespace {
 
@@ -243,11 +240,9 @@ static uav_status_t conv_out_launch(const void* x, int64_t B, int64_t T, int64_t
   UAV_REQUIRE(B > 0 && T > 0 && H > 0 && W > 0 && C == CO_C && ld >= C && ld % 8 == 0 && Cout >= 1 && Cout <= 5,
               "uav_conv_out_fused: needs C == 256 input channels and 1..5 output channels (C=%lld Cout=%lld)",
               (long long)C, (long long)Cout);
-  UAV_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(w) & 15) == 0,
-              "uav_conv_out_fused: x and w must be 16-byte aligned");
+  UAV_REQUIRE_ALIGNED16("uav_conv_out_fused", x);
+  UAV_REQUIRE_ALIGNED16("uav_conv_out_fused", w);
   UAV_REQUIRE(out_dtype == UAV_F16 || out_dtype == UAV_F32, "uav_conv_out_fused: bad out_dtype");
-  cudaStream_t stream_ = stream;
-  (void)stream_;
   ConvOutParams p;
   memset(&p, 0, sizeof(p));
   p.x = reinterpret_cast<const __half*>(x);
@@ -288,8 +283,7 @@ static uav_status_t conv_out_launch(const void* x, int64_t B, int64_t T, int64_t
   int64_t grid = num_sms();
   if (grid > p.num_tiles) grid = p.num_tiles;
   conv_out_fused_kernel<<<(unsigned)grid, CO_THREADS, SMEM, stream>>>(p);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 

@@ -5,18 +5,14 @@
 // timestep sinusoid (diffusers Timesteps, unet_video.py:173,472).
 #include "uav_common.cuh"
 
-#include <atomic>
-
 namespace uav {
-extern std::atomic<uint64_t> g_launches;
 
 // dst[p][0:C] = src[p][0:C]  (C % 8 == 0, 16-byte aligned)
 __global__ void __launch_bounds__(256)
     copy_channels_kernel(const __half* __restrict__ src, int64_t ld_src, __half* __restrict__ dst,
                          int64_t ld_dst, int octs, int64_t pixels) {
   const int64_t total = pixels * octs;
-  for (int64_t i = static_cast<int64_t>(blockIdx.x) * 256 + threadIdx.x; i < total;
-       i += static_cast<int64_t>(gridDim.x) * 256) {
+  UAV_GRID_STRIDE(i, total) {
     const int64_t p = i / octs;
     const int o = static_cast<int>(i - p * octs);
     stg16(dst + p * ld_dst + o * 8, ldg16(src + p * ld_src + o * 8));
@@ -31,8 +27,7 @@ __global__ void __launch_bounds__(256)
                             int64_t NB) {
   const int64_t total = NB * Ho * Wo * octs;
   const float sy = static_cast<float>(Hi) / Ho, sx = static_cast<float>(Wi) / Wo;
-  for (int64_t i = static_cast<int64_t>(blockIdx.x) * 256 + threadIdx.x; i < total;
-       i += static_cast<int64_t>(gridDim.x) * 256) {
+  UAV_GRID_STRIDE(i, total) {
     const int o = static_cast<int>(i % octs);
     int64_t r = i / octs;
     const int x = static_cast<int>(r % Wo);
@@ -52,8 +47,7 @@ __global__ void __launch_bounds__(256)
     planar_to_cl_kernel(const T* __restrict__ src, int C, int64_t thw, int64_t B,
                         __half* __restrict__ dst, int64_t ld_dst, int c_off, float scale) {
   const int64_t total = B * thw;
-  for (int64_t i = static_cast<int64_t>(blockIdx.x) * 256 + threadIdx.x; i < total;
-       i += static_cast<int64_t>(gridDim.x) * 256) {
+  UAV_GRID_STRIDE(i, total) {
     const int64_t b = i / thw, p = i - b * thw;
     for (int c = 0; c < C; ++c)
       dst[i * ld_dst + c_off + c] =
@@ -67,8 +61,7 @@ __global__ void __launch_bounds__(256)
     cl_to_planar_kernel(const TI* __restrict__ src, int64_t ld_src, int C, int64_t thw, int64_t B,
                         TO* __restrict__ dst, int clamp) {
   const int64_t total = B * thw;
-  for (int64_t i = static_cast<int64_t>(blockIdx.x) * 256 + threadIdx.x; i < total;
-       i += static_cast<int64_t>(gridDim.x) * 256) {
+  UAV_GRID_STRIDE(i, total) {
     const int64_t b = i / thw, p = i - b * thw;
     for (int c = 0; c < C; ++c) {
       float v = static_cast<float>(src[i * ld_src + c]);
@@ -80,8 +73,7 @@ __global__ void __launch_bounds__(256)
 
 __global__ void __launch_bounds__(256)
     silu_kernel(const __half* __restrict__ x, __half* __restrict__ y, int64_t n) {
-  for (int64_t i = static_cast<int64_t>(blockIdx.x) * 256 + threadIdx.x; i < n;
-       i += static_cast<int64_t>(gridDim.x) * 256)
+  UAV_GRID_STRIDE(i, n)
     y[i] = __float2half_rn(silu_f(__half2float(x[i])));
 }
 
@@ -91,8 +83,8 @@ __global__ void timestep_embedding_kernel(const float* __restrict__ t, int B, in
                                           int flip_sin_to_cos, float freq_shift,
                                           __half* __restrict__ out) {
   const int half = dim / 2;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < B * half; i += gridDim.x * blockDim.x) {
-    const int b = i / half, j = i % half;
+  UAV_GRID_STRIDE(i, B * half) {
+    const int b = static_cast<int>(i / half), j = static_cast<int>(i % half);
     const float f = expf(-logf(10000.f) * j / (half - freq_shift));
     const float a = t[b] * f;
     const float s = sinf(a), c = cosf(a);
@@ -106,8 +98,7 @@ __global__ void timestep_embedding_kernel(const float* __restrict__ t, int B, in
 __global__ void __launch_bounds__(256)
     sft_fuse_kernel(const __half* __restrict__ dec, const __half* __restrict__ scale,
                     const __half* __restrict__ shift, float w, float out_scale, __half* __restrict__ out, int64_t n8) {
-  for (int64_t i = static_cast<int64_t>(blockIdx.x) * 256 + threadIdx.x; i < n8;
-       i += static_cast<int64_t>(gridDim.x) * 256) {
+  UAV_GRID_STRIDE(i, n8) {
     const uint4 d = ldg16(dec + i * 8), sc = ldg16(scale + i * 8), sh = ldg16(shift + i * 8);
     const __half2* dh = reinterpret_cast<const __half2*>(&d);
     const __half2* ch = reinterpret_cast<const __half2*>(&sc);
@@ -123,14 +114,6 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-static inline unsigned grid_for(int64_t work, int per_thread = 4) {
-  int64_t g = (work + 256 * per_thread - 1) / (256 * per_thread);
-  const int64_t cap = static_cast<int64_t>(num_sms()) * 16;
-  if (g > cap) g = cap;
-  if (g < 1) g = 1;
-  return static_cast<unsigned>(g);
-}
-
 }  // namespace uav
 
 using namespace uav;
@@ -142,11 +125,13 @@ uav_status_t uav_copy_channels(const void* src, int64_t ld_src, void* dst, int64
   UAV_REQUIRE(src && dst && C > 0 && C % 8 == 0 && ld_src % 8 == 0 && ld_dst % 8 == 0 &&
                   ld_src >= C && ld_dst >= C,
               "uav_copy_channels: bad shape / alignment (C=%lld)", (long long)C);
+  UAV_REQUIRE(pixels >= 0, "uav_copy_channels: pixels must be >= 0");
+  UAV_REQUIRE_ALIGNED16("uav_copy_channels", src);
+  UAV_REQUIRE_ALIGNED16("uav_copy_channels", dst);
   if (pixels == 0) return UAV_OK;
-  copy_channels_kernel<<<grid_for(pixels * (C / 8)), 256, 0, (cudaStream_t)stream>>>(
+  copy_channels_kernel<<<stream_grid(pixels * (C / 8), 256 * 4, 16), 256, 0, (cudaStream_t)stream>>>(
       (const __half*)src, ld_src, (__half*)dst, ld_dst, (int)(C / 8), pixels);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
@@ -155,12 +140,16 @@ uav_status_t uav_upsample_nearest(const void* src, int64_t ld_src, int64_t NB, i
                                   int64_t Wo, uav_stream_t stream) {
   UAV_REQUIRE(src && dst && C > 0 && C % 8 == 0 && ld_src % 8 == 0 && ld_dst % 8 == 0,
               "uav_upsample_nearest: bad shape / alignment");
+  UAV_REQUIRE(ld_src >= C && ld_dst >= C, "uav_upsample_nearest: ld_src and ld_dst must be >= C");
   UAV_REQUIRE(NB > 0 && Hi > 0 && Wi > 0 && Ho > 0 && Wo > 0, "uav_upsample_nearest: bad shape");
-  upsample_nearest_kernel<<<grid_for(NB * Ho * Wo * (C / 8)), 256, 0, (cudaStream_t)stream>>>(
+  UAV_REQUIRE(Hi < (1 << 30) && Wi < (1 << 30) && Ho < (1 << 30) && Wo < (1 << 30),
+              "uav_upsample_nearest: Hi, Wi, Ho and Wo must be < 2^30");
+  UAV_REQUIRE_ALIGNED16("uav_upsample_nearest", src);
+  UAV_REQUIRE_ALIGNED16("uav_upsample_nearest", dst);
+  upsample_nearest_kernel<<<stream_grid(NB * Ho * Wo * (C / 8), 256 * 4, 16), 256, 0, (cudaStream_t)stream>>>(
       (const __half*)src, ld_src, (int)Hi, (int)Wi, (__half*)dst, ld_dst, (int)Ho, (int)Wo,
       (int)(C / 8), NB);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
@@ -169,15 +158,16 @@ uav_status_t uav_planar_to_channels_last(const void* src, int src_dtype, int64_t
                                          float scale, uav_stream_t stream) {
   UAV_REQUIRE(src && dst && B > 0 && C > 0 && thw > 0 && c_off >= 0 && c_off + C <= ld_dst,
               "uav_planar_to_channels_last: bad shape");
-  const unsigned g = grid_for(B * thw, 1);
+  UAV_REQUIRE(src_dtype == UAV_F16 || src_dtype == UAV_F32, "uav_planar_to_channels_last: unsupported src_dtype %d",
+              src_dtype);
+  const unsigned g = stream_grid(B * thw, 256, 16);
   if (src_dtype == UAV_F16)
     planar_to_cl_kernel<__half><<<g, 256, 0, (cudaStream_t)stream>>>(
         (const __half*)src, (int)C, thw, B, (__half*)dst, ld_dst, (int)c_off, scale);
   else
     planar_to_cl_kernel<float><<<g, 256, 0, (cudaStream_t)stream>>>(
         (const float*)src, (int)C, thw, B, (__half*)dst, ld_dst, (int)c_off, scale);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
@@ -186,7 +176,7 @@ uav_status_t uav_channels_last_to_planar(const void* src, int src_dtype, int64_t
                                          int clamp, uav_stream_t stream) {
   UAV_REQUIRE(src && dst && B > 0 && C > 0 && thw > 0 && ld_src >= C,
               "uav_channels_last_to_planar: bad shape");
-  const unsigned g = grid_for(B * thw, 1);
+  const unsigned g = stream_grid(B * thw, 256, 16);
   cudaStream_t s = (cudaStream_t)stream;
   if (src_dtype == UAV_F16 && dst_dtype == UAV_F16)
     cl_to_planar_kernel<__half, __half><<<g, 256, 0, s>>>((const __half*)src, ld_src, (int)C, thw,
@@ -201,17 +191,15 @@ uav_status_t uav_channels_last_to_planar(const void* src, int src_dtype, int64_t
     set_last_error("uav_channels_last_to_planar: unsupported dtype pair");
     return UAV_ERR_UNSUPPORTED;
   }
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
 uav_status_t uav_silu(const void* x, void* y, int64_t n, uav_stream_t stream) {
   UAV_REQUIRE(x && y && n >= 0, "uav_silu: bad argument");
   if (n == 0) return UAV_OK;
-  silu_kernel<<<grid_for(n, 1), 256, 0, (cudaStream_t)stream>>>((const __half*)x, (__half*)y, n);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  silu_kernel<<<stream_grid(n, 256, 16), 256, 0, (cudaStream_t)stream>>>((const __half*)x, (__half*)y, n);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
@@ -221,19 +209,21 @@ uav_status_t uav_timestep_embedding(const float* t, int64_t B, int64_t dim, int 
   timestep_embedding_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(t, (int)B, (int)dim,
                                                                 flip_sin_to_cos, freq_shift,
                                                                 (__half*)out);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
 uav_status_t uav_sft_fuse(const void* dec, const void* scale, const void* shift, float w, float out_scale, void* out,
                           int64_t n, uav_stream_t stream) {
   UAV_REQUIRE(dec && scale && shift && out && n >= 0 && n % 8 == 0, "uav_sft_fuse: bad argument");
+  UAV_REQUIRE_ALIGNED16("uav_sft_fuse", dec);
+  UAV_REQUIRE_ALIGNED16("uav_sft_fuse", scale);
+  UAV_REQUIRE_ALIGNED16("uav_sft_fuse", shift);
+  UAV_REQUIRE_ALIGNED16("uav_sft_fuse", out);
   if (n == 0) return UAV_OK;
-  sft_fuse_kernel<<<grid_for(n / 8), 256, 0, (cudaStream_t)stream>>>(
+  sft_fuse_kernel<<<stream_grid(n / 8, 256 * 4, 16), 256, 0, (cudaStream_t)stream>>>(
       (const __half*)dec, (const __half*)scale, (const __half*)shift, w, out_scale == 0.f ? 1.f : out_scale, (__half*)out, n / 8);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 

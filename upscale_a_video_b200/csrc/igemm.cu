@@ -512,8 +512,7 @@ static uav_status_t launch_instance2(IgemmParams& p, cudaStream_t stream) {
   if (st != UAV_OK) return st;
   const uint32_t sms = (uint32_t)num_sms();
   kern<<<p.num_tiles < sms ? p.num_tiles : sms, NUM_THREADS, Cfg::SMEM_BYTES, stream>>>(p);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
@@ -554,9 +553,7 @@ static uav_status_t launch_igemm(const IgemmDesc& d, const void* w, int64_t N, v
   UAV_REQUIRE(d.a && w && out, "igemm: null pointer");
   UAV_REQUIRE(d.k_per_tap > 0 && d.k_per_tap % 8 == 0,
               "igemm: input channels (%d) must be a positive multiple of 8", d.k_per_tap);
-  UAV_REQUIRE((reinterpret_cast<uintptr_t>(d.a) & 15) == 0 &&
-                  (reinterpret_cast<uintptr_t>(w) & 15) == 0,
-              "igemm: operands must be 16-byte aligned");
+  UAV_REQUIRE(aligned16(d.a) && aligned16(w), "igemm: operands must be 16-byte aligned");
   const bool geglu = e->act == UAV_ACT_GEGLU;
   UAV_REQUIRE(!geglu || (N % 128 == 0), "igemm: GEGLU needs N %% 128 == 0 (N=%lld)",
               (long long)N);
@@ -617,7 +614,6 @@ static uav_status_t launch_igemm(const IgemmDesc& d, const void* w, int64_t N, v
   p.n_tiles = (uint32_t)((p.n_out + out_tile_n - 1) / out_tile_n);
   UAV_REQUIRE(m_tiles * p.n_tiles < (1ull << 31), "igemm: too many tiles");
   p.num_tiles = (uint32_t)(m_tiles * p.n_tiles);
-  auto aligned16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
   const bool can_tma = out_tile_n >= 64 && e->out_dtype == UAV_F16 && p.n_out % 8 == 0 && e->ld_out % 8 == 0 &&
                        aligned16(out) &&
                        (e->residual == nullptr || (e->ld_res % 8 == 0 && aligned16(e->residual))) &&

@@ -8,12 +8,10 @@
 // AttentionBlock) is the same kernel with n_outer = b*t and pixels = h*w.
 #include "uav_common.cuh"
 
-#include <atomic>
 #include <limits.h>
 #include <string.h>
 
 namespace uav {
-extern std::atomic<uint64_t> g_launches;
 
 constexpr int GN_THREADS = 256;
 
@@ -427,15 +425,6 @@ size_t uav_groupnorm_workspace_bytes(int64_t n_outer, int groups) {
   return static_cast<size_t>(n_outer) * groups * (2 * sizeof(double) + GN_MAX_BLOCKS_PER_N * sizeof(float2));
 }
 
-// follows every GroupNorm launch: a launch error is returned, a launch that went in is counted
-#define GN_LAUNCHED()                                   \
-  do {                                                  \
-    UAV_CHECK_CUDA(cudaGetLastError());                 \
-    g_launches.fetch_add(1, std::memory_order_relaxed); \
-  } while (0)
-
-static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-
 // gridDim.x of a grid-stride pass over `items` per slab: about `per_sm` CTAs per SM over all n_outer slabs, at most one
 // per `per_block` items, at least one
 static int64_t gn_blocks(int per_sm, int64_t n_outer, int64_t items, int64_t per_block) {
@@ -461,9 +450,9 @@ static uav_status_t gn_stats_pass(const void* x, int64_t n_outer, int64_t pixels
     gn_stats_kernel<<<grid, GN_THREADS, 0, stream>>>(xh, pixels, (int)C, ld_in, groups, partial);
   else
     gn_stats_generic_kernel<<<grid, GN_THREADS, 0, stream>>>(xh, pixels, (int)C, ld_in, groups, partial);
-  GN_LAUNCHED();
+  UAV_LAUNCHED();
   gn_finalize_kernel<<<dim3((unsigned)groups, (unsigned)n_outer), 256, 0, stream>>>(partial, (int)gx, groups, sums);
-  GN_LAUNCHED();
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
@@ -511,7 +500,7 @@ static uav_status_t gn_reduce_sources(const GnReduceParams& prm, int64_t n_outer
                                       cudaStream_t stream) {
   gn_reduce_partials_kernel<<<dim3((unsigned)prm.G, (unsigned)n_outer, (unsigned)S), 256, 0, stream>>>(
       prm, reinterpret_cast<double*>(workspace));
-  GN_LAUNCHED();
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
@@ -525,7 +514,7 @@ static uav_status_t gn_apply(const void* x, int64_t n_outer, int64_t pixels, int
   gn_apply_vec_kernel<<<dim3((unsigned)gx, (unsigned)n_outer), GN_THREADS, 0, stream>>>(
       reinterpret_cast<const __half*>(x), pixels, (int)Cs, ld_in, groups, reinterpret_cast<const double*>(workspace), S,
       gamma, beta, eps, silu, reinterpret_cast<__half*>(y), ld_out, (int)C, chan, x_slab_stride);
-  GN_LAUNCHED();
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
@@ -553,7 +542,7 @@ uav_status_t uav_groupnorm_silu(const void* x, int64_t n_outer, int64_t pixels, 
                     2 * C * sizeof(float), stream>>>(reinterpret_cast<const __half*>(x), pixels, (int)C, ld_in, groups,
                                                      reinterpret_cast<const double*>(workspace), gamma, beta, eps, silu,
                                                      reinterpret_cast<__half*>(y), ld_out);
-  GN_LAUNCHED();
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
@@ -582,7 +571,7 @@ uav_status_t uav_groupnorm_affine(const void* x, int64_t n_outer, int64_t pixels
   gn_affine_kernel<<<dim3((unsigned)((C + 255) / 256), (unsigned)n_outer), 256, 0, stream>>>(
       reinterpret_cast<const double*>(workspace), S, groups, (int)C, static_cast<double>(pixels) * (C / groups), gamma,
       beta, eps, reinterpret_cast<float2*>(affine));
-  GN_LAUNCHED();
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
@@ -636,12 +625,13 @@ uav_status_t uav_layernorm(const void* x, int64_t rows, int64_t C, int64_t ld_in
   UAV_REQUIRE(rows >= 0 && C > 0 && C % 8 == 0 && C <= 2048 && ld_in >= C && ld_out >= C &&
                   ld_in % 8 == 0 && ld_out % 8 == 0,
               "uav_layernorm: bad shape (C=%lld)", (long long)C);
+  UAV_REQUIRE_ALIGNED16("uav_layernorm", x);
+  UAV_REQUIRE_ALIGNED16("uav_layernorm", y);
+  UAV_REQUIRE_ALIGNED16("uav_layernorm", gamma);
+  UAV_REQUIRE_ALIGNED16("uav_layernorm", beta);
   if (rows == 0) return UAV_OK;
   // grid-stride over tokens: 8 warps per block, at most 8 blocks per SM
-  int64_t blocks = (rows + 7) / 8;
-  const int64_t cap = (int64_t)num_sms() * 8;
-  if (blocks > cap) blocks = cap;
-  const unsigned grid = (unsigned)blocks;
+  const unsigned grid = stream_grid(rows, 8, 8);
   const int octs = (int)(C / 8);
   if (octs <= 64)
     layernorm_kernel<2, 2><<<grid, 256, 0, stream>>>(reinterpret_cast<const __half*>(x), rows, (int)C,
@@ -655,8 +645,7 @@ uav_status_t uav_layernorm(const void* x, int64_t rows, int64_t C, int64_t ld_in
     layernorm_kernel<8, 1><<<grid, 256, 0, stream>>>(reinterpret_cast<const __half*>(x), rows, (int)C,
                                                   ld_in, gamma, beta, eps,
                                                   reinterpret_cast<__half*>(y), ld_out);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 

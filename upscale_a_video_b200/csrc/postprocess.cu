@@ -12,23 +12,7 @@
 //     (not the telescoped image_0 - low_5, which rounds differently).
 #include "uav_common.cuh"
 
-#include <atomic>
-
 namespace uav {
-extern std::atomic<uint64_t> g_launches;
-int num_sms();
-
-#define UAV_PP_GRID_STRIDE(i, n)                                                      \
-  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < (n); \
-       i += static_cast<int64_t>(gridDim.x) * blockDim.x)
-
-static unsigned grid_for(int64_t n, int threads, int per_sm = 8) {
-  int64_t blocks = (n + threads - 1) / threads;
-  const int64_t cap = static_cast<int64_t>(num_sms()) * per_sm;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  return static_cast<unsigned>(blocks);
-}
 
 // ---------------------------------------------------------------------------------------
 // bicubic upsampling, align_corners=False, A=-0.75, border-clamped taps
@@ -48,7 +32,7 @@ __device__ __forceinline__ void cubic_coeffs(float t, float (&c)[4]) {
 __global__ void bicubic_kernel(const float* __restrict__ in, int64_t planes, int h, int w, int oh, int ow,
                                float scale_h, float scale_w, float* __restrict__ out) {
   const int64_t total = planes * oh * ow;
-  UAV_PP_GRID_STRIDE(i, total) {
+  UAV_GRID_STRIDE(i, total) {
     const int ox = static_cast<int>(i % ow);
     const int oy = static_cast<int>((i / ow) % oh);
     const int64_t pl = i / (static_cast<int64_t>(ow) * oh);
@@ -128,7 +112,7 @@ __global__ void adain_apply_kernel(const float* __restrict__ content, int64_t pl
                                    const float* __restrict__ s_mean, const float* __restrict__ s_std,
                                    float* __restrict__ out) {
   const int64_t total = planes * hw;
-  UAV_PP_GRID_STRIDE(i, total) {
+  UAV_GRID_STRIDE(i, total) {
     const int64_t pl = i / hw;
     const float n = __fdiv_rn(__fsub_rn(content[i], c_mean[pl]), c_std[pl]);
     out[i] = __fadd_rn(__fmul_rn(n, s_std[pl]), s_mean[pl]);
@@ -146,7 +130,7 @@ __global__ void wavelet_level_kernel(const float* __restrict__ img, int64_t plan
                                      const float* __restrict__ add) {
   const int64_t hw = static_cast<int64_t>(H) * W;
   const int64_t total = planes * hw;
-  UAV_PP_GRID_STRIDE(i, total) {
+  UAV_GRID_STRIDE(i, total) {
     const int x = static_cast<int>(i % W);
     const int y = static_cast<int>((i / W) % H);
     const float* src = img + (i / hw) * hw;
@@ -184,7 +168,7 @@ __global__ void wavelet_level_kernel(const float* __restrict__ img, int64_t plan
 template <bool PNG>
 __global__ void pack_uint8_kernel(const float* __restrict__ x, int64_t T, int C, int64_t hw, uint8_t* __restrict__ out) {
   const int64_t total = T * hw;
-  UAV_PP_GRID_STRIDE(i, total) {
+  UAV_GRID_STRIDE(i, total) {
     const int64_t t = i / hw, px = i % hw;
     const float* src = x + t * C * hw + px;
     uint8_t* dst = out + i * C;
@@ -225,7 +209,7 @@ __global__ void unpack_uint8_kernel(const uint8_t* __restrict__ in, int64_t T, i
                                     int64_t w_out, float* __restrict__ out) {
   const int64_t hw_out = h_out * w_out;
   const int64_t total = T * hw_out;
-  UAV_PP_GRID_STRIDE(i, total) {
+  UAV_GRID_STRIDE(i, total) {
     const int64_t ox = i % w_out, oy = (i / w_out) % h_out, t = i / hw_out;
     const int64_t y0 = area_start(oy, h_out, H), y1 = area_end(oy, h_out, H);
     const int64_t x0 = area_start(ox, w_out, W), x1 = area_end(ox, w_out, W);
@@ -258,9 +242,8 @@ uav_status_t uav_bicubic_upsample(const float* in, int64_t planes, int64_t h, in
   const int oh = static_cast<int>(h * scale), ow = static_cast<int>(w * scale);
   const int64_t total = planes * oh * ow;
   const float s = 1.0f / static_cast<float>(scale);  // scale_factor given -> ATen uses 1 / scale_factor
-  bicubic_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(in, planes, (int)h, (int)w, oh, ow, s, s, out);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  bicubic_kernel<<<stream_grid(total, 256, 8), 256, 0, (cudaStream_t)stream>>>(in, planes, (int)h, (int)w, oh, ow, s, s, out);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
@@ -272,25 +255,23 @@ uav_status_t uav_plane_stats(const float* x, int64_t planes, int64_t hw, float e
                              float* stdv, uav_stream_t stream) {
   UAV_REQUIRE(x && workspace && mean && stdv && planes > 0 && hw > 1, "uav_plane_stats: bad argument");
   UAV_REQUIRE(planes <= 65535, "uav_plane_stats: more than 65535 planes");
-  UAV_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 15) == 0, "uav_plane_stats: workspace must be 16-byte aligned");
+  UAV_REQUIRE_ALIGNED16("uav_plane_stats", workspace);
   double2* partial = reinterpret_cast<double2*>(workspace);
   plane_stats_partial_kernel<<<dim3(PS_BLOCKS_PER_PLANE, (unsigned)planes), PS_THREADS, 0, (cudaStream_t)stream>>>(
       x, hw, partial);
-  UAV_CHECK_CUDA(cudaGetLastError());
+  UAV_LAUNCHED();
   plane_stats_finalize_kernel<<<(unsigned)((planes + 63) / 64), 64, 0, (cudaStream_t)stream>>>(partial, planes, hw, eps,
                                                                                                mean, stdv);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(2, std::memory_order_relaxed);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
 uav_status_t uav_adain_apply(const float* content, int64_t planes, int64_t hw, const float* c_mean, const float* c_std,
                              const float* s_mean, const float* s_std, float* out, uav_stream_t stream) {
   UAV_REQUIRE(content && c_mean && c_std && s_mean && s_std && out && planes > 0 && hw > 0, "uav_adain_apply: bad argument");
-  adain_apply_kernel<<<grid_for(planes * hw, 256), 256, 0, (cudaStream_t)stream>>>(content, planes, hw, c_mean, c_std,
-                                                                                   s_mean, s_std, out);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  adain_apply_kernel<<<stream_grid(planes * hw, 256, 8), 256, 0, (cudaStream_t)stream>>>(content, planes, hw, c_mean, c_std,
+                                                                                          s_mean, s_std, out);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
@@ -300,28 +281,25 @@ uav_status_t uav_wavelet_level(const float* image, int64_t planes, int64_t H, in
   UAV_REQUIRE(H < (1 << 30) && W < (1 << 30), "uav_wavelet_level: frame too large");
   UAV_REQUIRE(low != nullptr || high != nullptr, "uav_wavelet_level: nothing to write");
   UAV_REQUIRE(low != image && high != image, "uav_wavelet_level: outputs must not alias the input (neighbour reads)");
-  wavelet_level_kernel<<<grid_for(planes * H * W, 256), 256, 0, (cudaStream_t)stream>>>(image, planes, (int)H, (int)W,
-                                                                                         radius, low, high, high_first, add);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  wavelet_level_kernel<<<stream_grid(planes * H * W, 256, 8), 256, 0, (cudaStream_t)stream>>>(image, planes, (int)H, (int)W,
+                                                                                              radius, low, high, high_first, add);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
 uav_status_t uav_pack_video_uint8(const float* frames, int64_t T, int64_t C, int64_t H, int64_t W, uint8_t* out,
                                   uav_stream_t stream) {
   UAV_REQUIRE(frames && out && T > 0 && C > 0 && C <= 4 && H > 0 && W > 0, "uav_pack_video_uint8: bad argument");
-  pack_uint8_kernel<false><<<grid_for(T * H * W, 256), 256, 0, (cudaStream_t)stream>>>(frames, T, (int)C, H * W, out);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  pack_uint8_kernel<false><<<stream_grid(T * H * W, 256, 8), 256, 0, (cudaStream_t)stream>>>(frames, T, (int)C, H * W, out);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
 uav_status_t uav_pack_frames_png(const float* frames, int64_t T, int64_t C, int64_t H, int64_t W, uint8_t* out,
                                  uav_stream_t stream) {
   UAV_REQUIRE(frames && out && T > 0 && C > 0 && C <= 4 && H > 0 && W > 0, "uav_pack_frames_png: bad argument");
-  pack_uint8_kernel<true><<<grid_for(T * H * W, 256), 256, 0, (cudaStream_t)stream>>>(frames, T, (int)C, H * W, out);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  pack_uint8_kernel<true><<<stream_grid(T * H * W, 256, 8), 256, 0, (cudaStream_t)stream>>>(frames, T, (int)C, H * W, out);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
@@ -334,13 +312,12 @@ uav_status_t uav_unpack_video_uint8(const uint8_t* frames, int64_t T, int64_t H,
   // torch reduces to a 1 x 1 output with a mean, whose summation order this kernel does not reproduce
   UAV_REQUIRE(h_out > 1 || w_out > 1 || (H == 1 && W == 1), "uav_unpack_video_uint8: a 1x1 output is not supported");
   UAV_REQUIRE(H < (1 << 30) && W < (1 << 30), "uav_unpack_video_uint8: frame too large");
-  const unsigned grid = grid_for(T * h_out * w_out, 256);
+  const unsigned grid = stream_grid(T * h_out * w_out, 256, 8);
   if (nhwc)
     unpack_uint8_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>(frames, T, H, W, h_out, w_out, out);
   else
     unpack_uint8_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(frames, T, H, W, h_out, w_out, out);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 

@@ -10,23 +10,7 @@
 // Activations are channels-last fp16 [pixel][C]; coordinates, the correlation volume and the flows are fp32.
 #include "uav_common.cuh"
 
-#include <atomic>
-
 namespace uav {
-extern std::atomic<uint64_t> g_launches;
-int num_sms();
-
-#define UAV_RAFT_GRID_STRIDE(i, n)                                                    \
-  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < (n); \
-       i += static_cast<int64_t>(gridDim.x) * blockDim.x)
-
-static unsigned raft_grid(int64_t n, int threads) {
-  int64_t blocks = (n + threads - 1) / threads;
-  const int64_t cap = static_cast<int64_t>(num_sms()) * 8;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  return static_cast<unsigned>(blocks);
-}
 
 // ---------------------------------------------------------------------------------------
 // InstanceNorm2d (no affine, biased variance, eps) + optional ReLU on [n][hw][C] fp16, C % 8 == 0, C <= 2048
@@ -96,7 +80,7 @@ __global__ void instnorm_finalize_kernel(const float2* __restrict__ partial, int
 __global__ void instnorm_apply_kernel(const __half* __restrict__ x, int64_t hw, int C, const float2* __restrict__ stats,
                                       int relu, __half* __restrict__ y, int64_t total_octs) {
   const int octs = C >> 3;
-  UAV_RAFT_GRID_STRIDE(i, total_octs) {
+  UAV_GRID_STRIDE(i, total_octs) {
     const int oct = static_cast<int>(i % octs);
     const int64_t pix = i / octs;
     const int64_t n = pix / hw;
@@ -122,7 +106,7 @@ __global__ void instnorm_apply_kernel(const __half* __restrict__ x, int64_t hw, 
 
 // y = relu(a + b), n8 groups of 8 halfs
 __global__ void add_relu_kernel(const __half* __restrict__ a, const __half* __restrict__ b, __half* __restrict__ y, int64_t n8) {
-  UAV_RAFT_GRID_STRIDE(i, n8) {
+  UAV_GRID_STRIDE(i, n8) {
     const uint4 va = ldg16(a + i * 8), vb = ldg16(b + i * 8);
     const __half2* ha = reinterpret_cast<const __half2*>(&va);
     const __half2* hb = reinterpret_cast<const __half2*>(&vb);
@@ -144,7 +128,7 @@ __global__ void split_tanh_relu_kernel(const __half* __restrict__ cnet, int64_t 
                                        int64_t ld_net, __half* __restrict__ inp_a, int64_t ld_a, __half* __restrict__ inp_b,
                                        int64_t ld_b) {
   const int64_t total = rows * C;
-  UAV_RAFT_GRID_STRIDE(i, total) {
+  UAV_GRID_STRIDE(i, total) {
     const int64_t r = i / C;
     const int c = static_cast<int>(i % C);
     const float a = __half2float(cnet[r * 2 * C + c]), b = __half2float(cnet[r * 2 * C + C + c]);
@@ -161,7 +145,7 @@ __global__ void split_tanh_relu_kernel(const __half* __restrict__ cnet, int64_t 
 __global__ void avgpool2_kernel(const float* __restrict__ in, int64_t planes, int h, int w, float* __restrict__ out) {
   const int oh = h / 2, ow = w / 2;
   const int64_t total = planes * oh * ow;
-  UAV_RAFT_GRID_STRIDE(i, total) {
+  UAV_GRID_STRIDE(i, total) {
     const int x = static_cast<int>(i % ow), y = static_cast<int>((i / ow) % oh);
     const int64_t pl = i / (static_cast<int64_t>(ow) * oh);
     const float* src = in + (pl * h + 2 * y) * w + 2 * x;
@@ -224,7 +208,7 @@ __global__ void __launch_bounds__(256)
 __global__ void gru_rh_kernel(const __half* __restrict__ zr, int64_t ld_zr, const __half* __restrict__ h, int64_t ld_h,
                               __half* __restrict__ out, int64_t ld_out, int64_t rows, int C) {
   const int64_t total = rows * C;
-  UAV_RAFT_GRID_STRIDE(i, total) {
+  UAV_GRID_STRIDE(i, total) {
     const int64_t r = i / C;
     const int c = static_cast<int>(i % C);
     out[r * ld_out + c] = __float2half_rn(__half2float(zr[r * ld_zr + C + c]) * __half2float(h[r * ld_h + c]));
@@ -233,7 +217,7 @@ __global__ void gru_rh_kernel(const __half* __restrict__ zr, int64_t ld_zr, cons
 __global__ void gru_update_kernel(const __half* __restrict__ zr, int64_t ld_zr, const __half* __restrict__ q, int64_t ld_q,
                                   __half* __restrict__ h, int64_t ld_h, int64_t rows, int C) {
   const int64_t total = rows * C;
-  UAV_RAFT_GRID_STRIDE(i, total) {
+  UAV_GRID_STRIDE(i, total) {
     const int64_t r = i / C;
     const int c = static_cast<int>(i % C);
     const float z = __half2float(zr[r * ld_zr + c]);
@@ -248,7 +232,7 @@ __global__ void gru_update_kernel(const __half* __restrict__ zr, int64_t ld_zr, 
 __global__ void flow_update_kernel(float* __restrict__ coords1, const float* __restrict__ delta, int64_t ld_delta, int64_t rows,
                                    int w8, int h8, __half* __restrict__ flow16, int64_t ld16, __half* __restrict__ dst_a,
                                    int64_t ld_a, __half* __restrict__ dst_b, int64_t ld_b) {
-  UAV_RAFT_GRID_STRIDE(r, rows) {
+  UAV_GRID_STRIDE(r, rows) {
     float cx = coords1[r * 2], cy = coords1[r * 2 + 1];
     if (delta != nullptr) {
       cx += delta[r * ld_delta];
@@ -279,7 +263,7 @@ __global__ void convex_upsample_kernel(const float* __restrict__ coords1, const 
                                        int64_t nimg, int h8, int w8, float* __restrict__ out) {
   const int H = 8 * h8, W = 8 * w8;
   const int64_t total = nimg * H * W;
-  UAV_RAFT_GRID_STRIDE(i, total) {
+  UAV_GRID_STRIDE(i, total) {
     const int X = static_cast<int>(i % W), Y = static_cast<int>((i / W) % H);
     const int64_t n = i / (static_cast<int64_t>(W) * H);
     const int ci = Y >> 3, a = Y & 7, cj = X >> 3, b = X & 7;
@@ -328,59 +312,63 @@ uav_status_t uav_instnorm_relu(const void* x, int64_t n, int64_t hw, int64_t C, 
                                uav_stream_t stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   UAV_REQUIRE(x && y && workspace && n > 0 && hw > 0, "uav_instnorm_relu: bad argument");
-  UAV_REQUIRE(C >= 8 && C % 8 == 0 && C <= 2048 && n <= 65535, "uav_instnorm_relu: C must be a multiple of 8 in [8, 2048]");
+  UAV_REQUIRE(C >= 8 && C % 8 == 0 && C <= 2048, "uav_instnorm_relu: C must be a multiple of 8 in [8, 2048]");
+  UAV_REQUIRE(n <= 65535, "uav_instnorm_relu: n must be at most 65535");
+  UAV_REQUIRE_ALIGNED16("uav_instnorm_relu", x);
+  UAV_REQUIRE_ALIGNED16("uav_instnorm_relu", y);
+  UAV_REQUIRE_ALIGNED16("uav_instnorm_relu", workspace);
   float2* partial = reinterpret_cast<float2*>(workspace);
   float2* stats = partial + n * IN_BLOCKS * C;
-  const int lanes = IN_THREADS / (int)(C / 8);
-  UAV_REQUIRE(lanes >= 1, "uav_instnorm_relu: too many channels");
-  const size_t smem = static_cast<size_t>(lanes) * C * 2 * sizeof(float);
-  if (smem > 48 * 1024)
-    UAV_CHECK_CUDA(cudaFuncSetAttribute(instnorm_stats_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  // lanes * C * 8 bytes = floor(256 / octs) * octs * 64 <= 16 KB: no opt-in needed
+  const size_t smem = static_cast<size_t>(IN_THREADS / (C / 8)) * C * 2 * sizeof(float);
   instnorm_stats_kernel<<<dim3(IN_BLOCKS, (unsigned)n), IN_THREADS, smem, stream>>>(reinterpret_cast<const __half*>(x), hw,
                                                                                    (int)C, partial);
-  UAV_CHECK_CUDA(cudaGetLastError());
+  UAV_LAUNCHED();
   instnorm_finalize_kernel<<<(unsigned)((n * C + 127) / 128), 128, 0, stream>>>(partial, n * C, (int)C, hw, eps, stats);
-  UAV_CHECK_CUDA(cudaGetLastError());
+  UAV_LAUNCHED();
   const int64_t total_octs = n * hw * (C / 8);
-  instnorm_apply_kernel<<<raft_grid(total_octs, 256), 256, 0, stream>>>(reinterpret_cast<const __half*>(x), hw, (int)C, stats,
-                                                                       relu, reinterpret_cast<__half*>(y), total_octs);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(3, std::memory_order_relaxed);
+  instnorm_apply_kernel<<<stream_grid(total_octs, 256, 8), 256, 0, stream>>>(reinterpret_cast<const __half*>(x), hw, (int)C,
+                                                                            stats, relu, reinterpret_cast<__half*>(y),
+                                                                            total_octs);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
 uav_status_t uav_add_relu(const void* a, const void* b, void* y, int64_t n, uav_stream_t stream) {
   UAV_REQUIRE(a && b && y && n > 0 && n % 8 == 0, "uav_add_relu: n must be a positive multiple of 8");
-  add_relu_kernel<<<raft_grid(n / 8, 256), 256, 0, (cudaStream_t)stream>>>(
+  UAV_REQUIRE_ALIGNED16("uav_add_relu", a);
+  UAV_REQUIRE_ALIGNED16("uav_add_relu", b);
+  UAV_REQUIRE_ALIGNED16("uav_add_relu", y);
+  add_relu_kernel<<<stream_grid(n / 8, 256, 8), 256, 0, (cudaStream_t)stream>>>(
       reinterpret_cast<const __half*>(a), reinterpret_cast<const __half*>(b), reinterpret_cast<__half*>(y), n / 8);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
 uav_status_t uav_raft_split_tanh_relu(const void* cnet, int64_t rows, int64_t C, void* net, int64_t ld_net, void* inp_a,
                                       int64_t ld_a, void* inp_b, int64_t ld_b, uav_stream_t stream) {
-  UAV_REQUIRE(cnet && net && inp_a && rows > 0 && C > 0, "uav_raft_split_tanh_relu: bad argument");
-  split_tanh_relu_kernel<<<raft_grid(rows * C, 256), 256, 0, (cudaStream_t)stream>>>(
+  UAV_REQUIRE(cnet && net && inp_a && rows > 0 && C > 0 && C <= INT32_MAX, "uav_raft_split_tanh_relu: bad argument");
+  UAV_REQUIRE(ld_net >= C && ld_a >= C && (inp_b == nullptr || ld_b >= C),
+              "uav_raft_split_tanh_relu: ld_net, ld_a and ld_b must be >= C");
+  split_tanh_relu_kernel<<<stream_grid(rows * C, 256, 8), 256, 0, (cudaStream_t)stream>>>(
       reinterpret_cast<const __half*>(cnet), rows, (int)C, reinterpret_cast<__half*>(net), ld_net,
       reinterpret_cast<__half*>(inp_a), ld_a, reinterpret_cast<__half*>(inp_b), ld_b);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
 uav_status_t uav_avgpool2x2_f32(const float* in, int64_t planes, int64_t h, int64_t w, float* out, uav_stream_t stream) {
   UAV_REQUIRE(in && out && planes > 0 && h >= 2 && w >= 2 && h < (1 << 20) && w < (1 << 20), "uav_avgpool2x2_f32: bad argument");
   const int64_t total = planes * (h / 2) * (w / 2);
-  avgpool2_kernel<<<raft_grid(total, 256), 256, 0, (cudaStream_t)stream>>>(in, planes, (int)h, (int)w, out);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  avgpool2_kernel<<<stream_grid(total, 256, 8), 256, 0, (cudaStream_t)stream>>>(in, planes, (int)h, (int)w, out);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
 uav_status_t uav_raft_corr_lookup(const float* const* levels, const int32_t* hs, const int32_t* ws, const float* coords,
                                   int64_t pixels, void* out, int64_t ld_out, uav_stream_t stream) {
   UAV_REQUIRE(levels && hs && ws && coords && out && pixels > 0 && ld_out >= 324, "uav_raft_corr_lookup: bad argument");
+  UAV_REQUIRE(ld_out <= INT32_MAX, "uav_raft_corr_lookup: ld_out must be < 2^31");
   LookupParams p;
   for (int i = 0; i < 4; ++i) {
     UAV_REQUIRE(levels[i] != nullptr && hs[i] >= 1 && ws[i] >= 1, "uav_raft_corr_lookup: bad pyramid level %d", i);
@@ -395,30 +383,32 @@ uav_status_t uav_raft_corr_lookup(const float* const* levels, const int32_t* hs,
   p.pad_from = 324;
   p.pad_to = (int)ld_out;
   corr_lookup_kernel<<<(unsigned)((pixels + 7) / 8), 256, 0, (cudaStream_t)stream>>>(p);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
 uav_status_t uav_raft_gru_rh(const void* zr, int64_t ld_zr, const void* h, int64_t ld_h, void* out, int64_t ld_out, int64_t rows,
                              int64_t C, uav_stream_t stream) {
-  UAV_REQUIRE(zr && h && out && rows > 0 && C > 0, "uav_raft_gru_rh: bad argument");
-  gru_rh_kernel<<<raft_grid(rows * C, 256), 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const __half*>(zr), ld_zr,
-                                                                            reinterpret_cast<const __half*>(h), ld_h,
-                                                                            reinterpret_cast<__half*>(out), ld_out, rows, (int)C);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  UAV_REQUIRE(zr && h && out && rows > 0 && C > 0 && C <= INT32_MAX, "uav_raft_gru_rh: bad argument");
+  UAV_REQUIRE(ld_zr >= 2 * C, "uav_raft_gru_rh: ld_zr must be >= 2C (the r half is read)");
+  UAV_REQUIRE(ld_h >= C && ld_out >= C, "uav_raft_gru_rh: ld_h and ld_out must be >= C");
+  gru_rh_kernel<<<stream_grid(rows * C, 256, 8), 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const __half*>(zr), ld_zr,
+                                                                                 reinterpret_cast<const __half*>(h), ld_h,
+                                                                                 reinterpret_cast<__half*>(out), ld_out, rows,
+                                                                                 (int)C);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
 uav_status_t uav_raft_gru_update(const void* zr, int64_t ld_zr, const void* q, int64_t ld_q, void* h, int64_t ld_h, int64_t rows,
                                  int64_t C, uav_stream_t stream) {
-  UAV_REQUIRE(zr && q && h && rows > 0 && C > 0, "uav_raft_gru_update: bad argument");
-  gru_update_kernel<<<raft_grid(rows * C, 256), 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const __half*>(zr), ld_zr,
-                                                                                reinterpret_cast<const __half*>(q), ld_q,
-                                                                                reinterpret_cast<__half*>(h), ld_h, rows, (int)C);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  UAV_REQUIRE(zr && q && h && rows > 0 && C > 0 && C <= INT32_MAX, "uav_raft_gru_update: bad argument");
+  UAV_REQUIRE(ld_zr >= C && ld_q >= C && ld_h >= C, "uav_raft_gru_update: ld_zr, ld_q and ld_h must be >= C");
+  gru_update_kernel<<<stream_grid(rows * C, 256, 8), 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const __half*>(zr),
+                                                                                     ld_zr, reinterpret_cast<const __half*>(q),
+                                                                                     ld_q, reinterpret_cast<__half*>(h), ld_h,
+                                                                                     rows, (int)C);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
@@ -426,22 +416,25 @@ uav_status_t uav_raft_flow_update(float* coords1, const float* delta, int64_t ld
                                   void* flow16, int64_t ld16, void* dst_a, int64_t ld_a, void* dst_b, int64_t ld_b,
                                   uav_stream_t stream) {
   UAV_REQUIRE(coords1 && rows > 0 && h8 > 0 && w8 > 0 && rows % (h8 * w8) == 0, "uav_raft_flow_update: bad argument");
-  flow_update_kernel<<<raft_grid(rows, 256), 256, 0, (cudaStream_t)stream>>>(coords1, delta, ld_delta, rows, (int)w8, (int)h8,
-                                                                             reinterpret_cast<__half*>(flow16), ld16,
-                                                                             reinterpret_cast<__half*>(dst_a), ld_a,
-                                                                             reinterpret_cast<__half*>(dst_b), ld_b);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  UAV_REQUIRE(h8 <= INT32_MAX && w8 <= INT32_MAX, "uav_raft_flow_update: h8 and w8 must be < 2^31");
+  UAV_REQUIRE((delta == nullptr || ld_delta >= 2) && (flow16 == nullptr || ld16 >= 2) && (dst_a == nullptr || ld_a >= 2) &&
+                  (dst_b == nullptr || ld_b >= 2),
+              "uav_raft_flow_update: ld_delta, ld16, ld_a and ld_b must be >= 2");
+  flow_update_kernel<<<stream_grid(rows, 256, 8), 256, 0, (cudaStream_t)stream>>>(coords1, delta, ld_delta, rows, (int)w8,
+                                                                                  (int)h8, reinterpret_cast<__half*>(flow16),
+                                                                                  ld16, reinterpret_cast<__half*>(dst_a), ld_a,
+                                                                                  reinterpret_cast<__half*>(dst_b), ld_b);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
 uav_status_t uav_raft_convex_upsample(const float* coords1, const void* mask, int64_t ld_mask, int64_t nimg, int64_t h8,
                                       int64_t w8, float* out, uav_stream_t stream) {
   UAV_REQUIRE(coords1 && mask && out && nimg > 0 && h8 > 0 && w8 > 0 && ld_mask >= 576, "uav_raft_convex_upsample: bad argument");
-  convex_upsample_kernel<<<raft_grid(nimg * 64 * h8 * w8, 256), 256, 0, (cudaStream_t)stream>>>(
+  UAV_REQUIRE(h8 < (1 << 28) && w8 < (1 << 28), "uav_raft_convex_upsample: h8 and w8 must be < 2^28 (8 h8 and 8 w8 are int)");
+  convex_upsample_kernel<<<stream_grid(nimg * 64 * h8 * w8, 256, 8), 256, 0, (cudaStream_t)stream>>>(
       coords1, reinterpret_cast<const __half*>(mask), ld_mask, nimg, (int)h8, (int)w8, out);
-  UAV_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 

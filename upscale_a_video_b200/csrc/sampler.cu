@@ -10,11 +10,7 @@
 // torch sequence while reading/writing each tensor once.
 #include "uav_common.cuh"
 
-#include <atomic>
-
 namespace uav {
-extern std::atomic<uint64_t> g_launches;
-
 template <bool HALF>
 struct Num;
 template <>
@@ -38,10 +34,6 @@ struct Num<false> {
   static __device__ __forceinline__ float add(float a, float b) { return __fadd_rn(a, b); }
   static __device__ __forceinline__ float sub(float a, float b) { return __fsub_rn(a, b); }
 };
-
-#define UAV_GRID_STRIDE(i, n)                                                         \
-  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < (n); \
-       i += static_cast<int64_t>(gridDim.x) * blockDim.x)
 
 // noise_pred = uncond + g * (text - uncond)   (pipeline_upscale_a_video.py:644-645)
 template <bool HALF>
@@ -267,14 +259,6 @@ __global__ void flow_resize_area_kernel(const void* in_, void* out_, int64_t pla
   }
 }
 
-static inline unsigned sgrid(int64_t n) {
-  int64_t g = (n + 255) / 256;
-  const int64_t cap = static_cast<int64_t>(num_sms()) * 16;
-  if (g > cap) g = cap;
-  if (g < 1) g = 1;
-  return static_cast<unsigned>(g);
-}
-
 }  // namespace uav
 
 using namespace uav;
@@ -287,8 +271,7 @@ using namespace uav;
       set_last_error("unsupported dtype %d", (int)(dtype));                                    \
       return UAV_ERR_INVALID;                                                                  \
     }                                                                                          \
-    UAV_CHECK_CUDA(cudaGetLastError());                                                        \
-    g_launches.fetch_add(1, std::memory_order_relaxed);                                        \
+    UAV_LAUNCHED();                                                                            \
   } while (0)
 
 extern "C" {
@@ -297,7 +280,7 @@ uav_status_t uav_cfg_combine(const void* pred2, void* out, int64_t n, float guid
                              int dtype, uav_stream_t stream) {
   UAV_REQUIRE(pred2 && out && n >= 0, "uav_cfg_combine: bad argument");
   if (n == 0) return UAV_OK;
-  UAV_DISPATCH_DTYPE(dtype, cfg_kernel, sgrid(n), stream, pred2, out, n, guidance_scale);
+  UAV_DISPATCH_DTYPE(dtype, cfg_kernel, stream_grid(n, 256, 16), stream, pred2, out, n, guidance_scale);
   return UAV_OK;
 }
 
@@ -307,7 +290,7 @@ uav_status_t uav_window_blend(void* dst, int64_t T, const void* src, int64_t Tw,
   UAV_REQUIRE(dst && src && T > 0 && Tw > 0 && Tw <= 32 && t0 >= 0 && t0 + Tw <= T && outer > 0 &&
                   hw > 0,
               "uav_window_blend: bad shape");
-  UAV_DISPATCH_DTYPE(dtype, window_blend_kernel, sgrid(outer * Tw * hw), stream, dst, T, src, Tw,
+  UAV_DISPATCH_DTYPE(dtype, window_blend_kernel, stream_grid(outer * Tw * hw, 256, 16), stream, dst, T, src, Tw,
                      (int)t0, covered_mask, outer, hw);
   return UAV_OK;
 }
@@ -318,7 +301,7 @@ uav_status_t uav_ddim_step_v0(const void* model_output, const void* sample, void
   UAV_REQUIRE(model_output && sample && x0 && n >= 0 && pred_type >= 0 && pred_type <= 2,
               "uav_ddim_step_v0: bad argument");
   if (n == 0) return UAV_OK;
-  UAV_DISPATCH_DTYPE(dtype, ddim_v0_kernel, sgrid(n), stream, model_output, sample, x0, n,
+  UAV_DISPATCH_DTYPE(dtype, ddim_v0_kernel, stream_grid(n, 256, 16), stream, model_output, sample, x0, n,
                      pred_type, sqrt_alpha, sqrt_beta, 1.0f / sqrt_alpha, clip, clip_range);
   return UAV_OK;
 }
@@ -331,7 +314,7 @@ uav_status_t uav_ddim_step_vt(const void* x0, const void* model_output, const vo
   UAV_REQUIRE(x0 && model_output && sample && prev && n >= 0 && pred_type >= 0 && pred_type <= 2,
               "uav_ddim_step_vt: bad argument");
   if (n == 0) return UAV_OK;
-  UAV_DISPATCH_DTYPE(dtype, ddim_vt_kernel, sgrid(n), stream, x0, model_output, sample, prev, n,
+  UAV_DISPATCH_DTYPE(dtype, ddim_vt_kernel, stream_grid(n, 256, 16), stream, x0, model_output, sample, prev, n,
                      pred_type, sqrt_alpha, sqrt_beta, 1.0f / sqrt_beta, sqrt_alpha_prev, dir_coef,
                      clip, clip_range, std_dev, noise);
   return UAV_OK;
@@ -342,7 +325,7 @@ uav_status_t uav_add_noise(const void* x, const void* noise, void* out, int64_t 
                            uav_stream_t stream) {
   UAV_REQUIRE(x && noise && out && n >= 0, "uav_add_noise: bad argument");
   if (n == 0) return UAV_OK;
-  UAV_DISPATCH_DTYPE(dtype, add_noise_kernel, sgrid(n), stream, x, noise, out, n, sqrt_alpha,
+  UAV_DISPATCH_DTYPE(dtype, add_noise_kernel, stream_grid(n, 256, 16), stream, x, noise, out, n, sqrt_alpha,
                      sqrt_one_minus_alpha);
   return UAV_OK;
 }
@@ -354,9 +337,10 @@ uav_status_t uav_propagate_step(const void* feat_prop, const void* feat_cur, con
                                 float alpha1, float alpha2, int dtype, uav_stream_t stream) {
   UAV_REQUIRE(feat_prop && feat_cur && flow_prop && flow_check && out && C > 0 && H > 0 && W > 0,
               "uav_propagate_step: bad argument");
+  UAV_REQUIRE(C <= INT32_MAX && H <= INT32_MAX && W <= INT32_MAX, "uav_propagate_step: C, H and W must be < 2^31");
   const float inv_wm1 = 1.0f / static_cast<float>(W > 1 ? W - 1 : 1);
   const float inv_hm1 = 1.0f / static_cast<float>(H > 1 ? H - 1 : 1);
-  UAV_DISPATCH_DTYPE(dtype, propagate_step_kernel, sgrid(H * W), stream, feat_prop, feat_cur,
+  UAV_DISPATCH_DTYPE(dtype, propagate_step_kernel, stream_grid(H * W, 256, 16), stream, feat_prop, feat_cur,
                      flow_prop, flow_check, out, (int)C, (int)H, (int)W, cs_prop, cs_cur, cs_out,
                      cs_flow_prop, cs_flow_check, nearest, fuse, fuse_scale, alpha1, alpha2, inv_wm1,
                      inv_hm1);
@@ -369,7 +353,7 @@ uav_status_t uav_flow_resize_area(const void* in, void* out, int64_t planes, int
   UAV_REQUIRE(in && out, "uav_flow_resize_area: null pointer");
   UAV_REQUIRE(planes > 0 && t_in > 0 && h_in > 0 && w_in > 0 && t_out > 0 && h_out > 0 && w_out > 0,
               "uav_flow_resize_area: bad shape");
-  UAV_DISPATCH_DTYPE(dtype, flow_resize_area_kernel, sgrid(planes * t_out * h_out * w_out), stream, in,
+  UAV_DISPATCH_DTYPE(dtype, flow_resize_area_kernel, stream_grid(planes * t_out * h_out * w_out, 256, 16), stream, in,
                      out, planes, t_in, h_in, w_in, t_out, h_out, w_out, scale);
   return UAV_OK;
 }

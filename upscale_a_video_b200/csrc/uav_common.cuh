@@ -318,8 +318,35 @@ __device__ __forceinline__ __half* tile_ptr(__half* base, int row, int chunk) {
 }
 
 // ---------------------------------------------------------------------------------------
-// launch plumbing (host)
+// launch plumbing
 // ---------------------------------------------------------------------------------------
+// i = every index in [0, n) that this thread owns in a grid-stride loop over a 1-D grid
+#define UAV_GRID_STRIDE(i, n)                                                         \
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < (n); \
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x)
+
+// gridDim.x of a grid-stride kernel over `items`: one block per `items_per_block`, at most `blocks_per_sm` blocks per SM,
+// at least one block
+inline unsigned stream_grid(int64_t items, int64_t items_per_block, int blocks_per_sm) {
+  int64_t blocks = (items + items_per_block - 1) / items_per_block;
+  const int64_t cap = static_cast<int64_t>(num_sms()) * blocks_per_sm;
+  if (blocks > cap) blocks = cap;
+  return static_cast<unsigned>(blocks < 1 ? 1 : blocks);
+}
+
+extern std::atomic<uint64_t> g_launches;  // kernels this library has launched: uav_launch_count()
+
+// follows every kernel launch: a launch error is returned, a launch that went in is counted
+#define UAV_LAUNCHED()                                       \
+  do {                                                       \
+    UAV_CHECK_CUDA(cudaGetLastError());                      \
+    uav::g_launches.fetch_add(1, std::memory_order_relaxed); \
+  } while (0)
+
+// 16-byte alignment, which ldg16 / stg16, float4 loads, cp.async and TMA need; a null pointer passes
+inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+#define UAV_REQUIRE_ALIGNED16(fn, ptr) UAV_REQUIRE(uav::aligned16(ptr), fn ": " #ptr " must be 16-byte aligned")
+
 // Encodes the tensor map of an fp16 tensor of `rank` <= 5 dims (dims and box innermost first, `strides` = the byte
 // strides of dims 1..rank-1) with the 128B swizzle that the wgmma operand tiles and the output staging use, unit element
 // strides and zero fill out of bounds.  `what` names the map in the error message.

@@ -607,10 +607,10 @@ def window_blend(dst: torch.Tensor, src: torch.Tensor, t0: int, covered_mask: in
     B, Cc, T, H, W = dst.shape
     Tw = src.shape[2]
     assert src.dtype == dst.dtype
+    _dt(src)
     lib = _lib.load()
     _lib.check(lib.uav_window_blend(dst.data_ptr(), T, src.data_ptr(), Tw, t0, covered_mask, B * Cc, H * W, _dt(dst),
                                     _stream()), "uav_window_blend")
-    _dt(src)
     return dst
 
 
