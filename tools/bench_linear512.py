@@ -1,13 +1,30 @@
 """Linear K=512 -> N=512 at M = 737 280 (the most frequent launch of a UNet forward: 39 of 319) alone, with and without
-the residual operand / statistics epilogue, inputs rotated past L2.  Prints ms, TFLOP/s and the HBM rate of the
-algorithmic bytes."""
-import os, sys
+the residual operand / statistics epilogue, the single-tap GEMMs of the default h720 clip (16 x 90x160, 45x80 and 23x40
+tokens per level, the VAE's 16 x 180x320 pixels), and the two few-wave h720 3x3 convolutions plus one many-wave one
+that WIDE_TILE_COST in igemm.cu is calibrated on.  Inputs rotated past L2.  Prints ms, TFLOP/s and the HBM rate of the
+algorithmic bytes, with the card and its power limit."""
+import os, subprocess, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from upscale_a_video_b200 import ops
 
 dev = torch.device("cuda")
 print({k: v for k, v in os.environ.items() if k.startswith("UAV_")})
+smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                     capture_output=True, text=True).stdout.strip()
+print(f"device: {torch.cuda.get_device_name()} | {smi}")
+
+
+def timed(one, iters):
+    for i in range(3):
+        one(i)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for i in range(iters):
+        one(i)
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / iters
 
 
 def run(M, K, N, residual, gn_stats, act=0, nbuf=3, iters=12):
@@ -21,18 +38,28 @@ def run(M, K, N, residual, gn_stats, act=0, nbuf=3, iters=12):
     def one(i):
         ops.linear(a[i % nbuf], w, b, out=outs[i % nbuf], residual=res[i % nbuf] if residual else None, act=act,
                    gn_stats=gn_stats)
-    for i in range(3):
-        one(i)
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for i in range(iters):
-        one(i)
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / iters
+    ms = timed(one, iters)
     gb = 2.0 * (M * K + M * n_out * (2 if residual else 1) + N * K) / 1e9
     print(f"linear M{M} K{K} N{N} act{act} residual={int(residual)} gn_stats={int(gn_stats)}: {ms * 1000:7.1f} us  "
           f"{2.0 * M * K * N / ms / 1e9:6.0f} TF/s  {gb / ms * 1000:6.0f} GB/s")
+
+
+def conv3x3(NB, H, W, Cin, Cout, slices=1, nbuf=3, iters=12):
+    """3x3 conv; slices > 1 runs it as that many launches of Cout / slices channels each (128 -> 128-column tiles)"""
+    x = [torch.randn(NB, H, W, Cin, device=dev).half() for _ in range(nbuf)]
+    w = (torch.randn(Cout, 3, 3, Cin, device=dev) * 0.02).half()
+    b = torch.zeros(Cout, device=dev)
+    outs = [torch.empty(NB, H, W, Cout, device=dev, dtype=torch.float16) for _ in range(nbuf)]
+    step = Cout // slices
+    ws = [w[s * step:(s + 1) * step].contiguous() for s in range(slices)]
+    bs = [b[s * step:(s + 1) * step].contiguous() for s in range(slices)]
+
+    def one(i):
+        for s in range(slices):
+            ops.conv2d(x[i % nbuf], ws[s], bs[s], out=outs[i % nbuf][..., s * step:(s + 1) * step])
+    ms = timed(one, iters)
+    print(f"conv3x3 {NB}x{H}x{W} {Cin}->{Cout} in {slices} launch(es): {ms * 1000:7.1f} us  "
+          f"{2.0 * NB * H * W * Cin * Cout * 9 / ms / 1e9:6.0f} TF/s")
 
 
 for residual, gn in ((False, False), (True, False), (True, True), (False, True)):
@@ -42,3 +69,15 @@ run(737280, 2048, 512, True, False)
 run(737280, 512, 4096, False, False, act=2)
 run(184320, 512, 512, True, False, nbuf=8, iters=32)
 run(46080, 1024, 1024, True, False, nbuf=16, iters=64)
+# h720: 16 x 90x160 tokens at level 1, 45x80 at level 2, 23x40 at level 3, the VAE at 16 x 180x320
+run(230400, 512, 512, False, False, nbuf=4, iters=24)
+run(230400, 512, 512, True, True, nbuf=4, iters=24)
+run(230400, 512, 1536, False, False, nbuf=4, iters=24)
+run(230400, 2048, 512, True, False, nbuf=4, iters=24)
+run(57600, 512, 512, True, False, nbuf=16, iters=64)
+run(14720, 1024, 1024, True, False, nbuf=16, iters=64)
+run(921600, 256, 256, True, False, nbuf=3, iters=12)
+conv3x3(16, 45, 80, 512, 512, iters=32)
+conv3x3(16, 23, 40, 1024, 1024, iters=32)
+conv3x3(16, 90, 160, 512, 512)
+conv3x3(16, 90, 160, 512, 512, slices=4)

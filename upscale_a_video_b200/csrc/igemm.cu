@@ -168,6 +168,19 @@ __device__ __forceinline__ float apply_act(float x, int act) {
     default: return x;
   }
 }
+// the activation of an epilogue body compiled for ACT: UAV_ACT_NONE (also GEGLU, which apply_act leaves alone), one
+// activation, or ACT_RUNTIME for the run-time `act`
+constexpr int ACT_RUNTIME = -1;
+template <int ACT>
+struct ActTag {
+  static constexpr int value = ACT;
+};
+template <int ACT>
+__device__ __forceinline__ float epi_act(float x, int act) {
+  if constexpr (ACT == UAV_ACT_NONE) return x;
+  else if constexpr (ACT == ACT_RUNTIME) return act != UAV_ACT_NONE ? apply_act(x, act) : x;
+  else return apply_act(x, ACT);
+}
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o >= 1; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -372,95 +385,106 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
     // each pass: an unrolled 256-column AUX epilogue would be twice the code and no longer fit the instruction cache.
     constexpr int EPI_N = GEGLU ? OUT_TILE_N : (OUT_TILE_N < 128 ? OUT_TILE_N : 128);
     constexpr int EPI_ACC = EPI_N / 2;
+    auto epilogue = [&](auto act_tag) {
+      [[maybe_unused]] constexpr int ACT = decltype(act_tag)::value;
 #pragma unroll 1
-    for (int pass = 0; pass < OUT_TILE_N / EPI_N; ++pass) {
+      for (int pass = 0; pass < OUT_TILE_N / EPI_N; ++pass) {
 #pragma unroll
-      for (int jb = 0; jb < EPI_N / 8; ++jb) {
-        const int col = pass * EPI_N + jb * 8 + 2 * lr;  // column inside the output tile (this thread: col, col + 1)
-        const int n = n_base + col;
-        const bool ok0 = n < p.n_out, ok1 = n + 1 < p.n_out;
-        float b0 = 0.f, b1 = 0.f, g0 = 0.f, g1 = 0.f;
-        if (p.bias != nullptr) {
-          if (ok0) b0 = __ldg(p.bias + n);
-          if (ok1) b1 = __ldg(p.bias + n + 1);
-          if (GEGLU) {
-            if (ok0) g0 = __ldg(p.bias + p.N / 2 + n);
-            if (ok1) g1 = __ldg(p.bias + p.N / 2 + n + 1);
+        for (int jb = 0; jb < EPI_N / 8; ++jb) {
+          const int col = pass * EPI_N + jb * 8 + 2 * lr;  // column inside the output tile (this thread: col, col + 1)
+          const int n = n_base + col;
+          const bool ok0 = n < p.n_out, ok1 = n + 1 < p.n_out;
+          float b0 = 0.f, b1 = 0.f, g0 = 0.f, g1 = 0.f;
+          if (p.bias != nullptr) {
+            if (ok0) b0 = __ldg(p.bias + n);
+            if (ok1) b1 = __ldg(p.bias + n + 1);
+            if (GEGLU) {
+              if (ok0) g0 = __ldg(p.bias + p.N / 2 + n);
+              if (ok1) g1 = __ldg(p.bias + p.N / 2 + n + 1);
+            }
           }
-        }
-        float gs = 0.f, gq = 0.f;  // GroupNorm statistics of this 8-column group over the thread's rows
+          float gs = 0.f, gq = 0.f;  // GroupNorm statistics of this 8-column group over the thread's rows
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const float a0 = acc[4 * jb + 2 * h], a1 = acc[4 * jb + 2 * h + 1];
-          float x0, x1;
-          if constexpr (GEGLU) {
-            constexpr int GJ = OUT_TILE_N / 8;  // gate columns start at accumulator column OUT_TILE_N
-            const float q0 = acc[4 * (jb + GJ) + 2 * h], q1 = acc[4 * (jb + GJ) + 2 * h + 1];
-            x0 = (a0 + b0) * gelu_erf_f(q0 + g0);
-            x1 = (a1 + b1) * gelu_erf_f(q1 + g1);
-          } else {
-            x0 = a0 + b0;
-            x1 = a1 + b1;
-          }
-          // staging address of (row, col): 16-byte chunk (col & 63) / 8 of the row, CU_TENSOR_MAP_SWIZZLE_128B
-          const uint32_t row = lrow[h];
-          uint8_t* sp = staging + (col >> 6) * SLAB_BYTES + row * 128 + ((((col & 63) >> 3) ^ (row & 7)) << 4) + (col & 7) * 2;
-          if constexpr (AUX) {
-            if (rv[h] != nullptr) {
-              if (ok0) x0 += __half2float(rv[h][n]);
-              if (ok1) x1 += __half2float(rv[h][n + 1]);
-            }
-            if (p.act != UAV_ACT_NONE) {
-              x0 = apply_act(x0, p.act);
-              x1 = apply_act(x1, p.act);
-            }
-            if (TMA_EPI && p.res_tma) {  // residual of this row from the staging tile (same swizzle as the store)
-              const float2 r = __half22float2(*reinterpret_cast<const __half2*>(sp));
-              x0 = fmaf(x0, p.out_scale, r.x);
-              x1 = fmaf(x1, p.out_scale, r.y);
-            } else if (res[h] != nullptr) {
-              x0 = fmaf(x0, p.out_scale, ok0 ? __half2float(res[h][n]) : 0.f);
-              x1 = fmaf(x1, p.out_scale, ok1 ? __half2float(res[h][n + 1]) : 0.f);
-            } else if (p.out_scale != 1.0f) {
-              x0 *= p.out_scale;
-              x1 *= p.out_scale;
-            }
-            if (row_ok[h] && ok0) {
-              gs += x0 + x1;
-              gq = fmaf(x0, x0, fmaf(x1, x1, gq));
-            }
-          }
-          if constexpr (TMA_EPI) {
-            *reinterpret_cast<uint32_t*>(sp) = pack_half2_sat(x0, x1);
-          } else if (row_ok[h]) {
-            if (p.out_dtype == UAV_F16) {
-              __half* op = reinterpret_cast<__half*>(p.out) + out_row[h] * p.ld_out + n;
-              if (ok0) op[0] = __float2half_rn(fminf(fmaxf(x0, -65504.f), 65504.f));
-              if (ok1) op[1] = __float2half_rn(fminf(fmaxf(x1, -65504.f), 65504.f));
+          for (int h = 0; h < 2; ++h) {
+            const float a0 = acc[4 * jb + 2 * h], a1 = acc[4 * jb + 2 * h + 1];
+            float x0, x1;
+            if constexpr (GEGLU) {
+              constexpr int GJ = OUT_TILE_N / 8;  // gate columns start at accumulator column OUT_TILE_N
+              const float q0 = acc[4 * (jb + GJ) + 2 * h], q1 = acc[4 * (jb + GJ) + 2 * h + 1];
+              x0 = (a0 + b0) * gelu_erf_f(q0 + g0);
+              x1 = (a1 + b1) * gelu_erf_f(q1 + g1);
             } else {
-              float* op = reinterpret_cast<float*>(p.out) + out_row[h] * p.ld_out + n;
-              if (ok0) op[0] = x0;
-              if (ok1) op[1] = x1;
+              x0 = a0 + b0;
+              x1 = a1 + b1;
+            }
+            // staging address of (row, col): 16-byte chunk (col & 63) / 8 of the row, CU_TENSOR_MAP_SWIZZLE_128B
+            const uint32_t row = lrow[h];
+            uint8_t* sp = staging + (col >> 6) * SLAB_BYTES + row * 128 + ((((col & 63) >> 3) ^ (row & 7)) << 4) + (col & 7) * 2;
+            if constexpr (AUX) {
+              if (rv[h] != nullptr) {
+                if (ok0) x0 += __half2float(rv[h][n]);
+                if (ok1) x1 += __half2float(rv[h][n + 1]);
+              }
+              x0 = epi_act<ACT>(x0, p.act);
+              x1 = epi_act<ACT>(x1, p.act);
+              if (TMA_EPI && p.res_tma) {  // residual of this row from the staging tile (same swizzle as the store)
+                const float2 r = __half22float2(*reinterpret_cast<const __half2*>(sp));
+                x0 = fmaf(x0, p.out_scale, r.x);
+                x1 = fmaf(x1, p.out_scale, r.y);
+              } else if (res[h] != nullptr) {
+                x0 = fmaf(x0, p.out_scale, ok0 ? __half2float(res[h][n]) : 0.f);
+                x1 = fmaf(x1, p.out_scale, ok1 ? __half2float(res[h][n + 1]) : 0.f);
+              } else if (p.out_scale != 1.0f) {
+                x0 *= p.out_scale;
+                x1 *= p.out_scale;
+              }
+              if (row_ok[h] && ok0) {
+                gs += x0 + x1;
+                gq = fmaf(x0, x0, fmaf(x1, x1, gq));
+              }
+            }
+            if constexpr (TMA_EPI) {
+              *reinterpret_cast<uint32_t*>(sp) = pack_half2_sat(x0, x1);
+            } else if (row_ok[h]) {
+              if (p.out_dtype == UAV_F16) {
+                __half* op = reinterpret_cast<__half*>(p.out) + out_row[h] * p.ld_out + n;
+                if (ok0) op[0] = __float2half_rn(fminf(fmaxf(x0, -65504.f), 65504.f));
+                if (ok1) op[1] = __float2half_rn(fminf(fmaxf(x1, -65504.f), 65504.f));
+              } else {
+                float* op = reinterpret_cast<float*>(p.out) + out_row[h] * p.ld_out + n;
+                if (ok0) op[0] = x0;
+                if (ok1) op[1] = x1;
+              }
+            }
+          }
+          if constexpr (AUX && TMA_EPI) {
+            if (p.gn_partial != nullptr) {  // warp-uniform: the 16 rows x 8 columns of this warp
+              gs = warp_sum(gs);
+              gq = warp_sum(gq);
+              const int oct = n >> 3;
+              const int64_t blk = static_cast<int64_t>(m_tile) * 8 + cw;
+              if (lane == 0 && blk < p.gn_blocks && oct * 8 < p.n_out) {
+                p.gn_partial[(static_cast<int64_t>(oct) * p.gn_blocks + blk) * 2] = gs;
+                p.gn_partial[(static_cast<int64_t>(oct) * p.gn_blocks + blk) * 2 + 1] = gq;
+              }
             }
           }
         }
-        if constexpr (AUX && TMA_EPI) {
-          if (p.gn_partial != nullptr) {  // warp-uniform: the 16 rows x 8 columns of this warp
-            gs = warp_sum(gs);
-            gq = warp_sum(gq);
-            const int oct = n >> 3;
-            const int64_t blk = static_cast<int64_t>(m_tile) * 8 + cw;
-            if (lane == 0 && blk < p.gn_blocks && oct * 8 < p.n_out) {
-              p.gn_partial[(static_cast<int64_t>(oct) * p.gn_blocks + blk) * 2] = gs;
-              p.gn_partial[(static_cast<int64_t>(oct) * p.gn_blocks + blk) * 2 + 1] = gq;
-            }
-          }
-        }
-      }
-      if (pass + 1 < OUT_TILE_N / EPI_N) {
+        if (pass + 1 < OUT_TILE_N / EPI_N) {
 #pragma unroll
-        for (int i = 0; i + EPI_ACC < Cfg::ACC; ++i) acc[i] = acc[i + EPI_ACC];
+          for (int i = 0; i + EPI_ACC < Cfg::ACC; ++i) acc[i] = acc[i + EPI_ACC];
+        }
       }
+    };
+    // The activation is the same for the whole launch, so it is picked here, once per tile, and each epilogue body is
+    // compiled for one activation: the run-time switch inlined at every element pair made the AUX epilogue several
+    // times as long as the one without activation, and launches without one or with SiLU pay for none of it.
+    if constexpr (AUX) {
+      if (p.act == UAV_ACT_SILU) epilogue(ActTag<UAV_ACT_SILU>{});
+      else if (p.act == UAV_ACT_NONE || p.act == UAV_ACT_GEGLU) epilogue(ActTag<UAV_ACT_NONE>{});
+      else epilogue(ActTag<ACT_RUNTIME>{});
+    } else {
+      epilogue(ActTag<UAV_ACT_NONE>{});
     }
     if constexpr (TMA_EPI) {
       // publish the staged tile to the async proxy and store it with TMA (clips OOB rows)
