@@ -681,16 +681,6 @@ uav_status_t attention_tc(const void* q, const void* k, const void* v, void* out
                           int64_t ldv, int64_t ldo, int64_t kv_batch_div, float scale,
                           cudaStream_t stream);  // attention_tc.cu (wgmma)
 
-// the opt-in, launch and launch check of flash_attn_kernel and every cross_attn_kernel
-template <auto Kernel>
-static uav_status_t launch_fa(const FaParams& p, dim3 grid, int smem, cudaStream_t stream) {
-  const uav_status_t st = opt_in_smem<Kernel>(smem);
-  if (st != UAV_OK) return st;
-  Kernel<<<grid, FA_THREADS, smem, stream>>>(p);
-  UAV_LAUNCHED();
-  return UAV_OK;
-}
-
 template <int D, int NB16>
 static uav_status_t launch_cross(const FaParams& p, int batch, cudaStream_t stream) {
   const int ntiles = (p.nq + FA_BM - 1) / FA_BM;
@@ -698,8 +688,8 @@ static uav_status_t launch_cross(const FaParams& p, int batch, cudaStream_t stre
   int gx = (num_sms() * 8 + batch * p.heads - 1) / (batch * p.heads);
   if (gx > ntiles) gx = ntiles;
   if (gx < 1) gx = 1;
-  return launch_fa<cross_attn_kernel<D, NB16>>(p, dim3(gx * p.heads, batch), (2 * NB16 * 16 * D + 2 * FA_BM * D) * 2,
-                                               stream);
+  return launch_opted_in<cross_attn_kernel<D, NB16>>(dim3(gx * p.heads, batch), FA_THREADS,
+                                                     (2 * NB16 * 16 * D + 2 * FA_BM * D) * 2, stream, p);
 }
 
 // blocks of 4 warps, one warp per (batch, pixel) and pair of heads (pairs) or head
@@ -754,8 +744,8 @@ uav_status_t uav_attention(const void* q, const void* k, const void* v, void* ou
     if (head_dim == 64) return nk <= 80 ? launch_cross<64, 5>(p, (int)batch, stream) : launch_cross<64, 8>(p, (int)batch, stream);
     return nk <= 80 ? launch_cross<128, 5>(p, (int)batch, stream) : launch_cross<128, 8>(p, (int)batch, stream);
   }
-  return launch_fa<flash_attn_kernel>(p, dim3((p.nq + FA_BM - 1) / FA_BM, batch * heads), (FA_BM + 4 * FA_BN) * FA_D * 2,
-                                      stream);
+  return launch_opted_in<flash_attn_kernel>(dim3((p.nq + FA_BM - 1) / FA_BM, batch * heads), FA_THREADS,
+                                            (FA_BM + 4 * FA_BN) * FA_D * 2, stream, p);
 }
 
 uav_status_t uav_temporal_attention(const void* q, const void* k, const void* v, void* out,

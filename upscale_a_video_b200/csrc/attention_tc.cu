@@ -40,7 +40,7 @@ struct FaTcCfg {
   static constexpr int Q_SLAB_BYTES = TC_BM * 128;
   static constexpr int Q_BYTES = QSLABS * Q_SLAB_BYTES;
   static constexpr int SLOT_BYTES = BN * 128;
-  static constexpr int STAGES_RAW = (232448 - 1024 - 1024 - Q_BYTES) / SLOT_BYTES;
+  static constexpr int STAGES_RAW = (SMEM_OPT_IN_LIMIT - 1024 - 1024 - Q_BYTES) / SLOT_BYTES;
   static constexpr int STAGES = STAGES_RAW > 16 ? 16 : STAGES_RAW;
   static_assert(STAGES >= 2, "ring does not fit");
   static constexpr int SMEM_BYTES = Q_BYTES + STAGES * SLOT_BYTES + 1024 + 1024;
@@ -54,14 +54,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
   constexpr int QSLABS = Cfg::QSLABS;
   constexpr int VBLKS = Cfg::VBLKS;
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw_addr = smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
-  uint8_t* sq = smem;
-  uint8_t* ring = sq + Cfg::Q_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ring + STAGES * Cfg::SLOT_BYTES);
-  uint64_t* full_bar = bars;                 // [STAGES]
-  uint64_t* empty_bar = bars + STAGES;       // [STAGES]: one arrival per consumer warp
-  uint64_t* q_bar = bars + 2 * STAGES;       // [1]
+  uint8_t* sq = smem_align1024(smem_raw);
+  uint8_t* slots = sq + Cfg::Q_BYTES;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(slots + STAGES * Cfg::SLOT_BYTES);
+  const RingBarriers<STAGES> ring(bars);
+  uint64_t* q_bar = bars + 2 * STAGES;
 
   const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * TC_BM;
@@ -75,10 +72,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     tma_prefetch_desc(&p.map_q);
     tma_prefetch_desc(&p.map_k);
     tma_prefetch_desc(&p.map_v);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 8);
-    }
+    ring.init(8);  // the 8 consumer warps
     mbar_init(q_bar, 1);
     fence_barrier_init();
   }
@@ -86,21 +80,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 
   if (warp_idx < 4) {
     // =============================== TMA producer ===============================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    setmaxnreg_dec<PRODUCER_REGS>();
     if (threadIdx.x == 0) {
       mbar_expect_tx(q_bar, Cfg::Q_BYTES);
       for (int c = 0; c < QSLABS; ++c)
         tma_load_3d(&p.map_q, q_bar, sq + c * Cfg::Q_SLAB_BYTES, h * DQK + c * 64, q0, b);
-      int stage = 0;
-      uint32_t phase = 0;
+      RingPos<STAGES> pos;
       auto load_slot = [&](const CUtensorMap* map, int col, int row) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        mbar_expect_tx(&full_bar[stage], Cfg::SLOT_BYTES);
-        tma_load_3d(map, &full_bar[stage], ring + stage * Cfg::SLOT_BYTES, col, row, bkv);
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
+        uint64_t* full = ring.acquire(pos, Cfg::SLOT_BYTES);
+        tma_load_3d(map, full, slots + pos.stage * Cfg::SLOT_BYTES, col, row, bkv);
+        pos.advance();
       };
       // same order as the consumers: K_j slots, then V_j slots
       for (int j = 0; j < ntiles; ++j) {
@@ -112,7 +101,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
   }
 
   // =============================== consumers: QK^T, softmax, PV, epilogue ===============================
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+  setmaxnreg_inc<CONSUMER_REGS>();
   const int wg = (threadIdx.x >> 7) - 1;  // query rows [64 wg, +64) of the CTA
   const int lq = lane >> 2, lr = lane & 3;
   float o[VBLKS][32];
@@ -121,32 +110,28 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 #pragma unroll
     for (int i = 0; i < 32; ++i) o[c][i] = 0.f;
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};  // rows lq and lq + 8 of this warp's 16
-  int stage = 0;
-  uint32_t phase = 0;
+  RingPos<STAGES> pos;
   mbar_wait(q_bar, 0);
 
   for (int j = 0; j < ntiles; ++j) {
     // ---- S = Q K_j^T ----
     float s[BN / 2];
-    const int k_first = stage;
+    const int k_first = pos.stage;
 #pragma unroll 1
     for (int c = 0; c < QSLABS; ++c) {
-      mbar_wait(&full_bar[stage], phase);
+      ring.wait_full(pos);
       const uint64_t adesc = gmma_desc_sw128(smem_u32(sq + c * Cfg::Q_SLAB_BYTES) + wg * (64 * 128));
-      const uint64_t bdesc = gmma_desc_sw128(smem_u32(ring + stage * Cfg::SLOT_BYTES));
+      const uint64_t bdesc = gmma_desc_sw128(smem_u32(slots + pos.stage * Cfg::SLOT_BYTES));
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < 4; ++k) wgmma_ss(s, adesc + 2 * k, bdesc + 2 * k, (c | k) != 0);
       wgmma_commit();
-      if (++stage == STAGES) {
-        stage = 0;
-        phase ^= 1;
-      }
+      pos.advance();
     }
     wgmma_wait<0>();
     wgmma_fence_operands(s);
     if (lane == 0)
-      for (int c = 0; c < QSLABS; ++c) mbar_arrive(&empty_bar[(k_first + c) % STAGES]);
+      for (int c = 0; c < QSLABS; ++c) mbar_arrive(&ring.empty[(k_first + c) % STAGES]);
 
     // ---- online softmax on the registers: s[i] is row lq + 8 ((i / 2) % 2), column 8 (i / 4) + 2 lr + i % 2 ----
     const int valid = p.nk - j * BN;  // columns >= valid are padding
@@ -188,26 +173,23 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
       }
 
     // ---- O += P V_j ----
-    const int v_first = stage;
+    const int v_first = pos.stage;
 #pragma unroll
     for (int c = 0; c < VBLKS; ++c) {
-      mbar_wait(&full_bar[stage], phase);
-      const uint64_t bdesc = gmma_desc_sw128(smem_u32(ring + stage * Cfg::SLOT_BYTES));
+      ring.wait_full(pos);
+      const uint64_t bdesc = gmma_desc_sw128(smem_u32(slots + pos.stage * Cfg::SLOT_BYTES));
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < BN / 16; ++kk)  // 16 kv rows per step: B + 16 rows * 128 B
         wgmma_rs_tb(o[c], pa[kk], bdesc + 128 * kk, 1u);
       wgmma_commit();
-      if (++stage == STAGES) {
-        stage = 0;
-        phase ^= 1;
-      }
+      pos.advance();
     }
     wgmma_wait<0>();
 #pragma unroll
     for (int c = 0; c < VBLKS; ++c) wgmma_fence_operands(o[c]);
     if (lane == 0)
-      for (int c = 0; c < VBLKS; ++c) mbar_arrive(&empty_bar[(v_first + c) % STAGES]);
+      for (int c = 0; c < VBLKS; ++c) mbar_arrive(&ring.empty[(v_first + c) % STAGES]);
   }
 
   // ---- epilogue: O / l -> global ----
@@ -234,13 +216,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 
 template <int DQK, int DVT, int BN>
 static uav_status_t launch_fa_tc(FaTcParams& p, int64_t batch, int dv_splits, cudaStream_t stream) {
-  using Cfg = FaTcCfg<DQK, DVT, BN>;
-  const uav_status_t st = opt_in_smem<fa_tc_kernel<DQK, DVT, BN>>(Cfg::SMEM_BYTES);
-  if (st != UAV_OK) return st;
-  dim3 grid((p.nq + TC_BM - 1) / TC_BM, dv_splits, (unsigned)(batch * p.heads));
-  fa_tc_kernel<DQK, DVT, BN><<<grid, TC_THREADS, Cfg::SMEM_BYTES, stream>>>(p);
-  UAV_LAUNCHED();
-  return UAV_OK;
+  const dim3 grid((p.nq + TC_BM - 1) / TC_BM, dv_splits, (unsigned)(batch * p.heads));
+  return launch_opted_in<fa_tc_kernel<DQK, DVT, BN>>(grid, TC_THREADS, FaTcCfg<DQK, DVT, BN>::SMEM_BYTES, stream, p);
 }
 
 

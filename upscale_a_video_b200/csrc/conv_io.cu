@@ -14,6 +14,7 @@
 // One persistent CTA per SM, 16 warps: tile = 14 x 30 output pixels -> 16 x 32 halo pixels = 32 m16 tiles (2 per warp);
 // K in 4 chunks of 64 channels, double buffered in shared memory, the next chunk's global loads in flight during the
 // MMAs of the current one.
+#include "sampler_math.cuh"
 #include "uav_common.cuh"
 
 #include <string.h>
@@ -53,12 +54,6 @@ struct ConvOutParams {
   __half* noise_pred;    // (1, Cout, T, H, W)
   __half* x0;            // (1, Cout, T, H, W)
 };
-
-// one torch op on fp16 tensors = fp32 math + one rounding to half (csrc/sampler.cu `Num<true>`): no FMA contraction
-__device__ __forceinline__ float rh16(float v) { return __half2float(__float2half_rn(v)); }
-__device__ __forceinline__ float mul16(float a, float b) { return rh16(__fmul_rn(a, b)); }
-__device__ __forceinline__ float add16(float a, float b) { return rh16(__fadd_rn(a, b)); }
-__device__ __forceinline__ float sub16(float a, float b) { return rh16(__fsub_rn(a, b)); }
 
 __global__ void __launch_bounds__(CO_THREADS, 1)
     conv_out_fused_kernel(const ConvOutParams p) {
@@ -202,18 +197,14 @@ __global__ void __launch_bounds__(CO_THREADS, 1)
         for (int kx = 0; kx < 3; ++kx)
           s += ys[((ly + ky) * CO_HW + lx + kx) * CO_YS + (ky * 3 + kx) * p.Cout + co];
       if (p.fuse_cfg) {
+        const float unet = Num<true>::rh(fminf(fmaxf(s, -65504.f), 65504.f));  // the UNet's fp16 output
         if (bi == 0) {
-          us[i] = rh16(fminf(fmaxf(s, -65504.f), 65504.f));  // the UNet's fp16 output, unconditional half
+          us[i] = unet;  // unconditional half
         } else {
-          const float u = us[i], c = rh16(fminf(fmaxf(s, -65504.f), 65504.f));
-          const float eps = add16(u, mul16(p.guidance, sub16(c, u)));
+          const float eps = cfg_combine<true>(us[i], unet, p.guidance);
           const int64_t o = (static_cast<int64_t>(co) * p.T + t) * plane + static_cast<int64_t>(gy) * p.W + gx;
-          const float smp = __half2float(p.sample[o]);
-          float r;
-          if (p.pred_type == 0) r = mul16(sub16(smp, mul16(p.sb, eps)), p.inv_sa);
-          else if (p.pred_type == 1) r = eps;
-          else r = sub16(mul16(p.sa, smp), mul16(p.sb, eps));
-          if (p.clip) r = fminf(fmaxf(r, -p.clip_range), p.clip_range);
+          const float r = ddim_x0<true>(eps, __half2float(p.sample[o]), p.pred_type, p.sa, p.sb, p.inv_sa, p.clip,
+                                        p.clip_range);
           p.noise_pred[o] = __float2half_rn(eps);
           p.x0[o] = __float2half_rn(r);
         }
@@ -278,13 +269,9 @@ static uav_status_t conv_out_launch(const void* x, int64_t B, int64_t T, int64_t
   }
   constexpr int SMEM = 2 * CO_XS_BYTES + CO_NPAD * CO_C * 2 + CO_TH * CO_TW * 5 * 4;
   static_assert(CO_PIX * CO_YS * 4 <= 2 * CO_XS_BYTES, "Y tile must fit in the activation buffers");
-  const uav_status_t st = opt_in_smem<conv_out_fused_kernel>(SMEM);
-  if (st != UAV_OK) return st;
   int64_t grid = num_sms();
   if (grid > p.num_tiles) grid = p.num_tiles;
-  conv_out_fused_kernel<<<(unsigned)grid, CO_THREADS, SMEM, stream>>>(p);
-  UAV_LAUNCHED();
-  return UAV_OK;
+  return launch_opted_in<conv_out_fused_kernel>((unsigned)grid, CO_THREADS, SMEM, stream, p);
 }
 
 uav_status_t uav_conv_out_fused(const void* x, int64_t B, int64_t T, int64_t H, int64_t W, int64_t C, int64_t ld,

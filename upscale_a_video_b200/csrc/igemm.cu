@@ -104,7 +104,6 @@ constexpr int NUM_THREADS = 384;      // warpgroup 0: TMA producer (one thread);
 constexpr int NUM_EPI_THREADS = 256;
 constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;
 constexpr int SLAB_BYTES = BLOCK_M * 128;  // 128 rows x 64 fp16 output columns, 128B-swizzled
-constexpr int SMEM_LIMIT = 232448;         // opt-in shared memory per block on sm_90 (227 KB)
 
 struct alignas(64) IgemmParams {
   CUtensorMap map_a;
@@ -146,16 +145,33 @@ struct IgemmCfg {
   static constexpr int STAGING_BYTES = (OUT_TILE_N >= 64) ? (OUT_TILE_N / 64) * SLAB_BYTES : 0;
   static constexpr int AUX_BYTES = 1024;  // mbarriers
   // everything left of the 227 KB after the output staging tile is the {A, B} stage ring
-  static constexpr int STAGES_RAW = (SMEM_LIMIT - 1024 - STAGING_BYTES - AUX_BYTES) / STAGE_BYTES;
+  static constexpr int STAGES_RAW = (SMEM_OPT_IN_LIMIT - 1024 - STAGING_BYTES - AUX_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + AUX_BYTES + 1024 /*align*/;
   static constexpr int ACC = BLOCK_N / 2;  // fp32 accumulator registers per thread: m64 x BLOCK_N per warpgroup
-  static_assert(SMEM_BYTES <= SMEM_LIMIT, "stage ring + output staging exceed the shared memory of a block");
+  static_assert(SMEM_BYTES <= SMEM_OPT_IN_LIMIT, "stage ring + output staging exceed the shared memory of a block");
 };
 
-__device__ __forceinline__ void epi_bar_sync() {
-  asm volatile("bar.sync 1, %0;" ::"n"(NUM_EPI_THREADS) : "memory");
+// The tile of work item w: its N-tile, its M-tile and the origin of the M-tile's box along view dims 1..4
+struct IgemmTile {
+  uint32_t n_tile, m_tile;
+  uint32_t t1, t2, t3, t4;
+};
+__device__ __forceinline__ IgemmTile igemm_tile(const IgemmParams& p, uint32_t w) {
+  IgemmTile t;
+  t.n_tile = w % p.n_tiles;
+  t.m_tile = w / p.n_tiles;
+  uint32_t idx = t.m_tile;
+  t.t1 = (idx % p.tiles[1]) * p.box[1];
+  idx /= p.tiles[1];
+  t.t2 = (idx % p.tiles[2]) * p.box[2];
+  idx /= p.tiles[2];
+  t.t3 = (idx % p.tiles[3]) * p.box[3];
+  idx /= p.tiles[3];
+  t.t4 = idx * p.box[4];
+  return t;
 }
+
 // pointwise activations of the fused epilogue (GEGLU is handled separately: it pairs two accumulator columns)
 __device__ __forceinline__ float apply_act(float x, int act) {
   switch (act) {
@@ -203,14 +219,11 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
   constexpr int OUT_TILE_N = Cfg::OUT_TILE_N;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment (SWIZZLE_128B atoms) in the shared address space
-  const uint32_t raw_addr = smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
+  uint8_t* smem = smem_align1024(smem_raw);
   uint8_t* staging = smem + STAGES * Cfg::STAGE_BYTES;
   uint64_t* bars = reinterpret_cast<uint64_t*>(staging + Cfg::STAGING_BYTES);
-  uint64_t* full_bar = bars;             // [STAGES]
-  uint64_t* empty_bar = bars + STAGES;   // [STAGES]: one arrival per consumer warp
-  uint64_t* res_bar = bars + 2 * STAGES; // residual tile landed in the staging tile
+  const RingBarriers<STAGES> ring(bars);  // one arrival per consumer warp on `empty`
+  uint64_t* res_bar = bars + 2 * STAGES;  // residual tile landed in the staging tile
 
   const int warp_idx = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -220,10 +233,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
     tma_prefetch_desc(&p.map_b);
     if (TMA_EPI) tma_prefetch_desc(&p.map_out);
     if (TMA_EPI && p.res_tma) tma_prefetch_desc(&p.map_res);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], NUM_EPI_THREADS / 32);
-    }
+    ring.init(NUM_EPI_THREADS / 32);
     mbar_init(res_bar, 1);
     fence_barrier_init();
   }
@@ -232,43 +242,29 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
 
   if (warp_idx < 4) {
     // =============================== TMA producer ===============================
-    // 128 x 40 + 256 x 232 registers fit the 64 K register file
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    setmaxnreg_dec<PRODUCER_REGS>();
     if (threadIdx.x == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
+      RingPos<STAGES> pos;
       for (uint32_t w = blockIdx.x; w < p.num_tiles; w += gridDim.x) {
-        const uint32_t n_tile = w % p.n_tiles;
-        uint32_t idx = w / p.n_tiles;
-        const int c1 = (idx % p.tiles[1]) * p.box[1];
-        idx /= p.tiles[1];
-        const int c2 = (idx % p.tiles[2]) * p.box[2];
-        idx /= p.tiles[2];
-        const int c3 = (idx % p.tiles[3]) * p.box[3];
-        idx /= p.tiles[3];
-        const int c4 = idx * p.box[4];
+        const IgemmTile t = igemm_tile(p, w);
         for (int tap = 0; tap < p.num_taps; ++tap) {
           const int o0 = p.tap_off[tap][0], o1 = p.tap_off[tap][1], o2 = p.tap_off[tap][2],
                     o3 = p.tap_off[tap][3], o4 = p.tap_off[tap][4];
           for (int kc = 0; kc < p.kblocks_per_tap; ++kc) {
-            mbar_wait(&empty_bar[stage], phase ^ 1);
-            uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
-            uint8_t* sb = sa + A_STAGE_BYTES;
             // out-of-bounds parts of a box (image border = zero padding, K tail, N tail) are zero-filled and counted
-            mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
-            tma_load_5d(&p.map_a, &full_bar[stage], sa, kc * BLOCK_K + o0, c1 + o1, c2 + o2, c3 + o3, c4 + o4);
+            uint64_t* full = ring.acquire(pos, Cfg::STAGE_BYTES);
+            uint8_t* sa = smem + pos.stage * Cfg::STAGE_BYTES;
+            uint8_t* sb = sa + A_STAGE_BYTES;
+            tma_load_5d(&p.map_a, full, sa, kc * BLOCK_K + o0, (int)t.t1 + o1, (int)t.t2 + o2, (int)t.t3 + o3,
+                        (int)t.t4 + o4);
             const int kcoord = tap * p.k_per_tap + kc * BLOCK_K;
             if (GEGLU) {  // value rows, then the matching gate rows
-              tma_load_2d(&p.map_b, &full_bar[stage], sb, kcoord, n_tile * (BLOCK_N / 2));
-              tma_load_2d(&p.map_b, &full_bar[stage], sb + Cfg::B_STAGE_BYTES / 2, kcoord,
-                          p.N / 2 + n_tile * (BLOCK_N / 2));
+              tma_load_2d(&p.map_b, full, sb, kcoord, t.n_tile * (BLOCK_N / 2));
+              tma_load_2d(&p.map_b, full, sb + Cfg::B_STAGE_BYTES / 2, kcoord, p.N / 2 + t.n_tile * (BLOCK_N / 2));
             } else {
-              tma_load_2d(&p.map_b, &full_bar[stage], sb, kcoord, n_tile * BLOCK_N);
+              tma_load_2d(&p.map_b, full, sb, kcoord, t.n_tile * BLOCK_N);
             }
-            if (++stage == STAGES) {
-              stage = 0;
-              phase ^= 1;
-            }
+            pos.advance();
           }
         }
       }
@@ -277,7 +273,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
   }
 
   // =============================== wgmma consumers + epilogue ===============================
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+  setmaxnreg_inc<CONSUMER_REGS>();
   const int et = threadIdx.x - 128;  // 0..255
   const int wg = et >> 7;            // rows [64 wg, +64) of the tile
   const int cw = et >> 5;            // rows [16 cw, +16): the accumulator rows of this warp
@@ -295,29 +291,20 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
     r /= p.box[3];
     l4[h] = r;
   }
-  int stage = 0;
-  uint32_t phase = 0, res_phase = 0;
+  RingPos<STAGES> pos;
+  uint32_t res_phase = 0;
   float acc[Cfg::ACC];
 #pragma unroll
   for (int i = 0; i < Cfg::ACC; ++i) acc[i] = 0.f;
 
   for (uint32_t w = blockIdx.x; w < p.num_tiles; w += gridDim.x) {
-    const uint32_t n_tile = w % p.n_tiles;
-    const uint32_t m_tile = w / p.n_tiles;
-    uint32_t idx = m_tile;
-    const uint32_t t1 = (idx % p.tiles[1]) * p.box[1];
-    idx /= p.tiles[1];
-    const uint32_t t2 = (idx % p.tiles[2]) * p.box[2];
-    idx /= p.tiles[2];
-    const uint32_t t3 = (idx % p.tiles[3]) * p.box[3];
-    idx /= p.tiles[3];
-    const uint32_t t4 = idx * p.box[4];
-    const int n_base = n_tile * OUT_TILE_N;
+    const IgemmTile tile = igemm_tile(p, w);
+    const int n_base = tile.n_tile * OUT_TILE_N;
 
     if constexpr (TMA_EPI) {
       if (et == 0) {
         // the store of the previous tile must have read the staging tile before it is refilled
-        asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+        tma_store_wait_read<0>();
         if (AUX && p.res_tma) {
           uint32_t bytes = 0;
 #pragma unroll
@@ -327,8 +314,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
 #pragma unroll
           for (int sl = 0; sl < OUT_TILE_N / 64; ++sl)
             if (n_base + sl * 64 < p.n_out)
-              tma_load_5d(&p.map_res, res_bar, staging + sl * SLAB_BYTES, n_base + sl * 64, (int)t1, (int)t2, (int)t3,
-                          (int)t4);
+              tma_load_5d(&p.map_res, res_bar, staging + sl * SLAB_BYTES, n_base + sl * 64, (int)tile.t1,
+                          (int)tile.t2, (int)tile.t3, (int)tile.t4);
         }
       }
     }
@@ -336,9 +323,9 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
     // ---- main loop: one stage = 4 k16 steps; the stage of step kb - 1 is released once step kb is in flight ----
     int prev = 0;
     for (int kb = 0; kb < num_kb; ++kb) {
-      mbar_wait(&full_bar[stage], phase);
-      const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES) + wg * (64 * 128);
-      const uint32_t sb = smem_u32(smem + stage * Cfg::STAGE_BYTES + A_STAGE_BYTES);
+      ring.wait_full(pos);
+      const uint32_t sa = smem_u32(smem + pos.stage * Cfg::STAGE_BYTES) + wg * (64 * 128);
+      const uint32_t sb = smem_u32(smem + pos.stage * Cfg::STAGE_BYTES + A_STAGE_BYTES);
       const uint64_t adesc = gmma_desc_sw128(sa), bdesc = gmma_desc_sw128(sb);
       wgmma_fence();
 #pragma unroll
@@ -346,17 +333,14 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
       wgmma_commit();
       if (kb > 0) {
         wgmma_wait<1>();
-        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+        if (lane == 0) mbar_arrive(&ring.empty[prev]);
       }
-      prev = stage;
-      if (++stage == STAGES) {
-        stage = 0;
-        phase ^= 1;
-      }
+      prev = pos.stage;
+      pos.advance();
     }
     wgmma_wait<0>();
     wgmma_fence_operands(acc);
-    if (lane == 0) mbar_arrive(&empty_bar[prev]);
+    if (lane == 0) mbar_arrive(&ring.empty[prev]);
 
     // ---- epilogue ----
     bool row_ok[2];
@@ -365,7 +349,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
     const __half* res[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const uint32_t o1 = t1 + l1[h], o2 = t2 + l2[h], o3 = t3 + l3[h], o4 = t4 + l4[h];
+      const uint32_t o1 = tile.t1 + l1[h], o2 = tile.t2 + l2[h], o3 = tile.t3 + l3[h], o4 = tile.t4 + l4[h];
       row_ok[h] = o1 < p.out_dims[1] && o2 < p.out_dims[2] && o3 < p.out_dims[3] && o4 < p.out_dims[4];
       out_row[h] = ((static_cast<int64_t>(o4) * p.out_dims[3] + o3) * p.out_dims[2] + o2) * p.out_dims[1] + o1;
       rv[h] = (AUX && p.rowvec != nullptr && row_ok[h]) ? p.rowvec + (out_row[h] / p.rows_per_vec) * p.ld_rowvec
@@ -373,7 +357,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
       res[h] = (AUX && !TMA_EPI && p.residual != nullptr && row_ok[h]) ? p.residual + out_row[h] * p.ld_res : nullptr;
     }
     if constexpr (TMA_EPI) {
-      epi_bar_sync();  // thread 0 saw the previous store release the staging tile
+      bar_sync<1, NUM_EPI_THREADS>();  // thread 0 saw the previous store release the staging tile
       if constexpr (AUX) {
         if (p.res_tma) {
           mbar_wait(res_bar, res_phase);
@@ -462,7 +446,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
               gs = warp_sum(gs);
               gq = warp_sum(gq);
               const int oct = n >> 3;
-              const int64_t blk = static_cast<int64_t>(m_tile) * 8 + cw;
+              const int64_t blk = static_cast<int64_t>(tile.m_tile) * 8 + cw;
               if (lane == 0 && blk < p.gn_blocks && oct * 8 < p.n_out) {
                 p.gn_partial[(static_cast<int64_t>(oct) * p.gn_blocks + blk) * 2] = gs;
                 p.gn_partial[(static_cast<int64_t>(oct) * p.gn_blocks + blk) * 2 + 1] = gq;
@@ -489,23 +473,18 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
     if constexpr (TMA_EPI) {
       // publish the staged tile to the async proxy and store it with TMA (clips OOB rows)
       fence_proxy_async();
-      epi_bar_sync();
+      bar_sync<1, NUM_EPI_THREADS>();
       if (et == 0) {
 #pragma unroll
-        for (int sl = 0; sl < OUT_TILE_N / 64; ++sl) {
-          if (n_base + sl * 64 < p.n_out) {
-            asm volatile(
-                "cp.async.bulk.tensor.5d.global.shared::cta.bulk_group"
-                " [%0, {%2, %3, %4, %5, %6}], [%1];" ::"l"(reinterpret_cast<uint64_t>(&p.map_out)),
-                "r"(smem_u32(staging + sl * SLAB_BYTES)), "r"(n_base + sl * 64), "r"(t1), "r"(t2), "r"(t3), "r"(t4)
-                : "memory");
-          }
-        }
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+        for (int sl = 0; sl < OUT_TILE_N / 64; ++sl)
+          if (n_base + sl * 64 < p.n_out)
+            tma_store_5d(&p.map_out, staging + sl * SLAB_BYTES, n_base + sl * 64, (int)tile.t1, (int)tile.t2,
+                         (int)tile.t3, (int)tile.t4);
+        tma_store_commit();
       }
     }
   }
-  if (TMA_EPI && et == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+  if (TMA_EPI && et == 0) tma_store_wait_read<0>();
 }
 
 // ---------------------------------------------------------------------------------------
@@ -528,29 +507,22 @@ struct IgemmDesc {
   uint64_t out_strides[5] = {};
 };
 
-template <int BLOCK_N, bool GEGLU, bool TMA_EPI, bool AUX>
-static uav_status_t launch_instance2(IgemmParams& p, cudaStream_t stream) {
-  using Cfg = IgemmCfg<BLOCK_N, GEGLU>;
-  constexpr auto kern = igemm_kernel<BLOCK_N, GEGLU, TMA_EPI, AUX>;
-  const uav_status_t st = opt_in_smem<kern>(Cfg::SMEM_BYTES);
-  if (st != UAV_OK) return st;
-  const uint32_t sms = (uint32_t)num_sms();
-  kern<<<p.num_tiles < sms ? p.num_tiles : sms, NUM_THREADS, Cfg::SMEM_BYTES, stream>>>(p);
-  UAV_LAUNCHED();
-  return UAV_OK;
-}
-
+// persistent launch: one CTA per SM, or per tile when there are fewer tiles
 template <int BLOCK_N, bool GEGLU>
 static uav_status_t launch_instance(IgemmParams& p, cudaStream_t stream) {
+  using Cfg = IgemmCfg<BLOCK_N, GEGLU>;
+  constexpr int smem = Cfg::SMEM_BYTES;
+  const uint32_t sms = (uint32_t)num_sms();
+  const dim3 grid(p.num_tiles < sms ? p.num_tiles : sms);
   const bool aux = p.rowvec != nullptr || p.residual != nullptr || (p.act != UAV_ACT_NONE && p.act != UAV_ACT_GEGLU) ||
                    p.out_scale != 1.0f || p.gn_partial != nullptr;
-  if constexpr (IgemmCfg<BLOCK_N, GEGLU>::OUT_TILE_N >= 64) {
+  if constexpr (Cfg::OUT_TILE_N >= 64) {
     if (p.tma_store) {
-      return aux ? launch_instance2<BLOCK_N, GEGLU, true, true>(p, stream)
-                 : launch_instance2<BLOCK_N, GEGLU, true, false>(p, stream);
+      return aux ? launch_opted_in<igemm_kernel<BLOCK_N, GEGLU, true, true>>(grid, NUM_THREADS, smem, stream, p)
+                 : launch_opted_in<igemm_kernel<BLOCK_N, GEGLU, true, false>>(grid, NUM_THREADS, smem, stream, p);
     }
   }
-  return launch_instance2<BLOCK_N, GEGLU, false, true>(p, stream);
+  return launch_opted_in<igemm_kernel<BLOCK_N, GEGLU, false, true>>(grid, NUM_THREADS, smem, stream, p);
 }
 
 // Time of one 256-column tile over one 128-column tile of the same GEMM (GEGLU: 128 over 64 output columns), from

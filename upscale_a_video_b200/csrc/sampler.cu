@@ -3,49 +3,21 @@
 // split DDIM step (step_v0 / step_vt), add_noise and flow-guided latent propagation with its
 // area resize of the flows.
 //
-// These run on the reference's own "b c t h w" latents (4 channels).  In fp16 the reference
-// rounds after EVERY torch op (0-dim fp32 scalars x fp16 CUDA tensors -> fp16; SURVEY.md
-// Appendix B), so each kernel replays that exact op sequence with a round-to-half after each
-// step (`rh`), in one launch instead of 3-10: results are bit-identical to the op-by-op
+// These run on the reference's own "b c t h w" latents (4 channels).  In fp16 each kernel
+// replays the reference's exact op sequence with a round-to-half after each step (Num<true>,
+// sampler_math.cuh), in one launch instead of 3-10: results are bit-identical to the op-by-op
 // torch sequence while reading/writing each tensor once.
-#include "uav_common.cuh"
+#include "sampler_math.cuh"
 
 namespace uav {
-template <bool HALF>
-struct Num;
-template <>
-struct Num<true> {
-  using T = __half;
-  static __device__ __forceinline__ float ld(const __half* p, int64_t i) { return __half2float(p[i]); }
-  static __device__ __forceinline__ void st(__half* p, int64_t i, float v) { p[i] = __float2half_rn(v); }
-  static __device__ __forceinline__ float rh(float v) { return __half2float(__float2half_rn(v)); }
-  static __device__ __forceinline__ float mul(float a, float b) { return rh(__fmul_rn(a, b)); }
-  static __device__ __forceinline__ float add(float a, float b) { return rh(__fadd_rn(a, b)); }
-  static __device__ __forceinline__ float sub(float a, float b) { return rh(__fsub_rn(a, b)); }
-};
-template <>
-struct Num<false> {
-  using T = float;
-  static __device__ __forceinline__ float ld(const float* p, int64_t i) { return p[i]; }
-  static __device__ __forceinline__ void st(float* p, int64_t i, float v) { p[i] = v; }
-  static __device__ __forceinline__ float rh(float v) { return v; }
-  // one torch op == one rounding: intrinsics keep nvcc from contracting a*b+c into an FMA
-  static __device__ __forceinline__ float mul(float a, float b) { return __fmul_rn(a, b); }
-  static __device__ __forceinline__ float add(float a, float b) { return __fadd_rn(a, b); }
-  static __device__ __forceinline__ float sub(float a, float b) { return __fsub_rn(a, b); }
-};
 
-// noise_pred = uncond + g * (text - uncond)   (pipeline_upscale_a_video.py:644-645)
 template <bool HALF>
 __global__ void cfg_kernel(const void* pred2_, void* out_, int64_t n, float g) {
   using N = Num<HALF>;
   const typename N::T* pred2 = reinterpret_cast<const typename N::T*>(pred2_);
   typename N::T* out = reinterpret_cast<typename N::T*>(out_);
   UAV_GRID_STRIDE(i, n) {
-    const float u = N::ld(pred2, i), t = N::ld(pred2, n + i);
-    const float d = N::sub(t, u);
-    const float m = N::mul(g, d);
-    N::st(out, i, N::add(u, m));
+    N::st(out, i, cfg_combine<HALF>(N::ld(pred2, i), N::ld(pred2, n + i), g));
   }
 }
 
@@ -73,7 +45,7 @@ __global__ void window_blend_kernel(void* dst_, int64_t T, const void* src_, int
   }
 }
 
-// DDIMScheduler.step_v0 (scheduling_ddim.py:383-433).  pred_type: 0 epsilon, 1 sample, 2 v
+// DDIMScheduler.step_v0
 template <bool HALF>
 __global__ void ddim_v0_kernel(const void* mo_, const void* x_, void* x0_, int64_t n, int pred_type,
                                float sa, float sb, float inv_sa, int clip, float clip_range) {
@@ -82,18 +54,7 @@ __global__ void ddim_v0_kernel(const void* mo_, const void* x_, void* x0_, int64
   const typename N::T* x = reinterpret_cast<const typename N::T*>(x_);
   typename N::T* x0 = reinterpret_cast<typename N::T*>(x0_);
   UAV_GRID_STRIDE(i, n) {
-    const float m = N::ld(mo, i), s = N::ld(x, i);
-    float r;
-    if (pred_type == 0) {
-      // (sample - beta^0.5 * eps) / alpha^0.5 ; CUDA divides by a CPU scalar as mul-by-reciprocal
-      r = N::mul(N::sub(s, N::mul(sb, m)), inv_sa);
-    } else if (pred_type == 1) {
-      r = m;
-    } else {
-      r = N::sub(N::mul(sa, s), N::mul(sb, m));
-    }
-    if (clip) r = fminf(fmaxf(r, -clip_range), clip_range);
-    N::st(x0, i, r);
+    N::st(x0, i, ddim_x0<HALF>(N::ld(mo, i), N::ld(x, i), pred_type, sa, sb, inv_sa, clip, clip_range));
   }
 }
 

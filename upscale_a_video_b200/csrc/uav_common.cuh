@@ -9,6 +9,7 @@
 #include <stdint.h>
 
 #include <atomic>
+#include <utility>
 
 #include "../../include/uav_b200.h"
 
@@ -106,7 +107,89 @@ __device__ __forceinline__ void tma_load_5d(const void* desc, uint64_t* bar, voi
       "r"(c3), "r"(c4)
       : "memory");
 }
+// shared -> global store of a box, in the bulk group that the next tma_store_commit() closes
+__device__ __forceinline__ void tma_store_5d(const void* desc, const void* smem, int c0, int c1, int c2, int c3,
+                                             int c4) {
+  asm volatile(
+      "cp.async.bulk.tensor.5d.global.shared::cta.bulk_group"
+      " [%0, {%2, %3, %4, %5, %6}], [%1];" ::"l"(reinterpret_cast<uint64_t>(desc)),
+      "r"(smem_u32(smem)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
+      : "memory");
+}
+__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// waits until at most N committed store groups still have to read their shared memory
+template <int N>
+__device__ __forceinline__ void tma_store_wait_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
 
+// ---- warp-specialised TMA -> wgmma pipelines ----
+constexpr int SMEM_OPT_IN_LIMIT = 232448;  // opt-in shared memory per block on sm_90 (227 KB)
+// Register split of a 384-thread block with one producer and two consumer warpgroups: 128 x 40 + 256 x 232 fit the
+// 64 K register file.
+constexpr int PRODUCER_REGS = 40;
+constexpr int CONSUMER_REGS = 232;
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N) : "memory");
+}
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N) : "memory");
+}
+
+// dynamic shared memory rounded up to 1024 bytes (the SWIZZLE_128B atom) in the shared address space
+__device__ __forceinline__ uint8_t* smem_align1024(uint8_t* smem_raw) {
+  const uint32_t raw_addr = smem_u32(smem_raw);
+  return smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
+}
+
+// named barrier ID over the first THREADS threads that reach it
+template <int ID, int THREADS>
+__device__ __forceinline__ void bar_sync() {
+  asm volatile("bar.sync %0, %1;" ::"n"(ID), "n"(THREADS) : "memory");
+}
+
+// Position in a ring of STAGES slots.  The phase flips at every wrap: a slot's barrier completes once per pass.
+template <int STAGES>
+struct RingPos {
+  uint32_t phase = 0;
+  int stage = 0;
+  __device__ __forceinline__ void advance() {
+    if (++stage == STAGES) {
+      stage = 0;
+      phase ^= 1;
+    }
+  }
+};
+
+// The mbarriers of a ring of STAGES shared-memory slots, filled by TMA and drained by consumer warps: the 2 * STAGES
+// barriers at `bars`.  Each consumer warp releases a slot with one mbar_arrive(&empty[stage]) from its lane 0 once its
+// MMAs have read it.
+template <int STAGES>
+struct RingBarriers {
+  uint64_t* full;   // [STAGES]: the slot's TMA bytes have landed
+  uint64_t* empty;  // [STAGES]: every consumer warp has released the slot
+  __device__ __forceinline__ explicit RingBarriers(uint64_t* bars) : full(bars), empty(bars + STAGES) {}
+  // one thread, before fence_barrier_init()
+  __device__ __forceinline__ void init(uint32_t consumer_warps) const {
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], consumer_warps);
+    }
+  }
+  // producer: waits for the consumers to release the slot at `pos`, then arms its full barrier for `bytes` of TMA loads
+  // and returns it
+  __device__ __forceinline__ uint64_t* acquire(const RingPos<STAGES>& pos, uint32_t bytes) const {
+    mbar_wait(&empty[pos.stage], pos.phase ^ 1);
+    mbar_expect_tx(&full[pos.stage], bytes);
+    return &full[pos.stage];
+  }
+  // consumer: waits for the slot at `pos` to be filled
+  __device__ __forceinline__ void wait_full(const RingPos<STAGES>& pos) const {
+    mbar_wait(&full[pos.stage], pos.phase);
+  }
+};
 
 // ---- wgmma (sm_90a warpgroup MMA) ----
 // All four warps of a warpgroup execute these.  The accumulator fragment of m64nNk16 (fp32) in thread t of the
@@ -364,6 +447,17 @@ uav_status_t opt_in_smem(int bytes) {
     UAV_CHECK_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
     configured.fetch_or(dev_bit, std::memory_order_relaxed);
   }
+  return UAV_OK;
+}
+
+// Launches Kernel<<<grid, threads, smem, stream>>>(args...) with `smem` bytes of dynamic shared memory opted in, and
+// checks the launch.
+template <auto Kernel, class... A>
+uav_status_t launch_opted_in(dim3 grid, int threads, int smem, cudaStream_t stream, A&&... args) {
+  const uav_status_t st = opt_in_smem<Kernel>(smem);
+  if (st != UAV_OK) return st;
+  Kernel<<<grid, threads, smem, stream>>>(std::forward<A>(args)...);
+  UAV_LAUNCHED();
   return UAV_OK;
 }
 
