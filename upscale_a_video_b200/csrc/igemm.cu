@@ -197,10 +197,28 @@ __device__ __forceinline__ float epi_act(float x, int act) {
   else if constexpr (ACT == ACT_RUNTIME) return act != UAV_ACT_NONE ? apply_act(x, act) : x;
   else return apply_act(x, ACT);
 }
-__device__ __forceinline__ float warp_sum(float v) {
+// Sums each of the NV values of a lane over the 32 lanes of the warp (NV a power of two <= 32) and returns sum number
+// lane >> (5 - log2 NV).  Recursive halving: at the step of offset o a lane keeps the half of its values that bit o of
+// its lane index picks and adds its partner's partial of that half, so the warp shuffles NV - 1 times (plus once per
+// step left over when NV < 32) instead of 5 NV times.  Each partial adds the same two lanes' partials as the butterfly
+// v += shfl_xor(v, o), o = 16 .. 1, so every sum is bitwise the butterfly's.
+template <int NV, int O = 16>
+__device__ __forceinline__ float warp_sum_transpose(float (&v)[NV], int lane) {
+  static_assert(NV >= 1 && NV <= 32 && (NV & (NV - 1)) == 0, "NV must be a power of two <= 32");
+  constexpr int HALF = NV * O / 32;  // values a lane still holds after this step
+  if constexpr (HALF >= 1) {
+    const bool upper = (lane & O) != 0;
 #pragma unroll
-  for (int o = 16; o >= 1; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
+    for (int i = 0; i < HALF; ++i) {
+      const float send = upper ? v[i] : v[i + HALF];
+      const float keep = upper ? v[i + HALF] : v[i];
+      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, O);
+    }
+  } else {
+    v[0] += __shfl_xor_sync(0xffffffffu, v[0], O);
+  }
+  if constexpr (O > 1) return warp_sum_transpose<NV, O / 2>(v, lane);
+  else return v[0];
 }
 
 // TMA_EPI: smem-staged TMA-store epilogue (aligned fp16 output, >= 64-column tiles) vs direct per-element stores.
@@ -373,6 +391,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
       [[maybe_unused]] constexpr int ACT = decltype(act_tag)::value;
 #pragma unroll 1
       for (int pass = 0; pass < OUT_TILE_N / EPI_N; ++pass) {
+        // GroupNorm statistics of 8-column group jb over the thread's rows: sum at [2 jb], sum of squares at [2 jb + 1]
+        [[maybe_unused]] float stats[EPI_N / 4];
 #pragma unroll
         for (int jb = 0; jb < EPI_N / 8; ++jb) {
           const int col = pass * EPI_N + jb * 8 + 2 * lr;  // column inside the output tile (this thread: col, col + 1)
@@ -442,16 +462,21 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
             }
           }
           if constexpr (AUX && TMA_EPI) {
-            if (p.gn_partial != nullptr) {  // warp-uniform: the 16 rows x 8 columns of this warp
-              gs = warp_sum(gs);
-              gq = warp_sum(gq);
-              const int oct = n >> 3;
-              const int64_t blk = static_cast<int64_t>(tile.m_tile) * 8 + cw;
-              if (lane == 0 && blk < p.gn_blocks && oct * 8 < p.n_out) {
-                p.gn_partial[(static_cast<int64_t>(oct) * p.gn_blocks + blk) * 2] = gs;
-                p.gn_partial[(static_cast<int64_t>(oct) * p.gn_blocks + blk) * 2 + 1] = gq;
-              }
-            }
+            stats[2 * jb] = gs;
+            stats[2 * jb + 1] = gq;
+          }
+        }
+        if constexpr (AUX && TMA_EPI) {
+          if (p.gn_partial != nullptr) {  // warp-uniform: the 16 rows x 8 columns of this warp per column group
+            // lane l ends up with the warp's sum of stats[l >> SHIFT]
+            constexpr int SHIFT = EPI_N == 128 ? 0 : 1;
+            static_assert(EPI_N / 4 == (32 >> SHIFT), "one statistics value per 2^SHIFT lanes");
+            const float s = warp_sum_transpose(stats, lane);
+            const int value = lane >> SHIFT;
+            const int oct = ((n_base + pass * EPI_N) >> 3) + (value >> 1);
+            const int64_t blk = static_cast<int64_t>(tile.m_tile) * 8 + cw;
+            if ((lane & ((1 << SHIFT) - 1)) == 0 && blk < p.gn_blocks && oct * 8 < p.n_out)
+              p.gn_partial[(static_cast<int64_t>(oct) * p.gn_blocks + blk) * 2 + (value & 1)] = s;
           }
         }
         if (pass + 1 < OUT_TILE_N / EPI_N) {
