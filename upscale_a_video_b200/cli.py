@@ -5,9 +5,11 @@ The reference's `inference_upscale_a_video.py` with its flags, defaults and outp
     python -m upscale_a_video_b200 -i inputs/clip.mp4 -o results -p 24,26,28 --color_fix Wavelet
 
 Per clip: uint8 frames are copied to the GPU and normalised (and area-downsampled by 4 when both sides are >= 1280) by
-`ops.unpack_video_uint8`; RAFT flows when `-p` is given; the pipeline, whole or tiled (`tiling.upscale_tiled`); the colour
-fix; uint8 packing on the GPU for the mp4 (`pack_video_uint8`) and, with `--save_image`, for the PNG frames
-(`pack_frames_png`, save_image's rounding).  Under `torchrun` (WORLD_SIZE > 1) each process drives the GPU LOCAL_RANK
+`ops.unpack_video_uint8`; RAFT flows when `-p` is given; the pipeline's sampling, whole or per tile
+(`tiling.iter_upscale_tiled`); then, 3 frames at a time, the decode, the colour fix, uint8 packing on the GPU for the
+mp4 (`pack_video_uint8`) and, with `--save_image`, for the PNG frames (`pack_frames_png`, save_image's rounding), and the
+writes.  No buffer at output resolution holds more than one 3-frame chunk, so memory does not grow with clip length
+beyond the low-resolution sampling state.  Under `torchrun` (WORLD_SIZE > 1) each process drives the GPU LOCAL_RANK
 and the pipeline's tile / window sharding splits the work; only rank 0 writes files.
 
 Deliberate differences from the reference CLI (INTEGRATION.md §3): there is no LLaVA captioner (`--caption` supplies
@@ -16,9 +18,10 @@ mp4v, and the tiling decision is taken per clip."""
 from __future__ import annotations
 
 import argparse
+import contextlib
 import os
 import time
-from typing import List, Optional
+from typing import Iterator, List, Optional, Tuple
 
 import numpy as np
 import torch
@@ -137,8 +140,12 @@ def load_models(args: argparse.Namespace, paths: dict, device):
     return pipeline.to(device), raft
 
 
-def upscale_clip(pipeline, raft, vframes: torch.Tensor, args: argparse.Namespace, prompt: str) -> torch.Tensor:
-    """inference_upscale_a_video.py:190-333: (1, 3, t, h, w) LR clip -> colour-fixed (t, 3, 4h, 4w) frames in [-1, 1]"""
+def upscale_clip(pipeline, raft, vframes: torch.Tensor, args: argparse.Namespace, prompt: str,
+                 fix_colors: bool = True) -> Iterator[Tuple[int, int, torch.Tensor]]:
+    """inference_upscale_a_video.py:190-333, 3 frames at a time: samples the (1, 3, t, h, w) LR clip, then yields
+    `(s, e, frames)` in time order, `frames` the colour-fixed (e - s, 3, 4h, 4w) output of frames [s, e) in [-1, 1].
+    Ranks that write nothing pass `fix_colors=False` (and get the decoded (1, 3, e - s, 4h, 4w) chunks): they only
+    have to take part in the collectives that run inside the iteration."""
     flows_bi = list(raft.forward_slicing(vframes)) if raft is not None else None
     _, _, _, h, w = vframes.shape
     generator = torch.Generator(device=vframes.device).manual_seed(SEED)
@@ -146,12 +153,15 @@ def upscale_clip(pipeline, raft, vframes: torch.Tensor, args: argparse.Namespace
                   noise_level=args.noise_level, negative_prompt=args.n_prompt,
                   propagation_steps=args.propagation_steps)
     if args.perform_tile or tiling.needs_tiling(h, w):
-        output = tiling.upscale_tiled(pipeline, vframes, flows_bi, generator, tile_size=args.tile_size,
-                                      overlap=TILE_OVERLAP, prompt=prompt, **kwargs)
+        chunks = tiling.iter_upscale_tiled(pipeline, vframes, flows_bi, generator, tile_size=args.tile_size,
+                                           overlap=TILE_OVERLAP, prompt=prompt, **kwargs)
     else:
-        with torch.no_grad():
-            output = pipeline(prompt, image=vframes, flows_bi=flows_bi, generator=generator, **kwargs).images
-    return color_correction.color_fix_frames(output, vframes, args.color_fix)
+        sampled = pipeline.sample_latents(prompt, image=vframes, flows_bi=flows_bi, generator=generator, **kwargs)
+        chunks = pipeline.decode_chunks(sampled)
+    for s, e, chunk in chunks:
+        if fix_colors:
+            chunk = color_correction.color_fix_frames(chunk, vframes[:, :, s:e], args.color_fix)
+        yield s, e, chunk
 
 
 def _init_distributed():
@@ -185,20 +195,34 @@ def main(argv: Optional[List[str]] = None) -> List[str]:
             index_str = f"[{i + 1}/{len(video_list)}]"
             log(f"{index_str} Processing video: ", video_name)
             vframes = ingest_frames(frames, device, from_video=video_io.is_video(video_path))
+            video_path_out, frame_dir = output_paths(args, video_name)
+            writer = None
+            if rank == 0:
+                os.makedirs(os.path.dirname(video_path_out), exist_ok=True)
+                writer = video_io.VideoWriter(video_path_out, fps, (4 * vframes.shape[-2], 4 * vframes.shape[-1]))
             torch.cuda.synchronize(device)
-            start = time.time()
-            output = upscale_clip(pipeline, raft, vframes, args, args.caption + args.a_prompt)
-            video = color_correction.pack_video_uint8(output).cpu().numpy()
-            png = color_correction.pack_frames_png(output).cpu().numpy() if args.save_image else None
-            torch.cuda.synchronize(device)
-            run_time = time.time() - start
+            start, write_time = time.time(), 0.0
+            try:
+                with writer or contextlib.nullcontext():
+                    for s, _, output in upscale_clip(pipeline, raft, vframes, args, args.caption + args.a_prompt,
+                                                     fix_colors=rank == 0):
+                        if writer is None:
+                            continue
+                        video = color_correction.pack_video_uint8(output).cpu().numpy()
+                        png = color_correction.pack_frames_png(output).cpu().numpy() if args.save_image else None
+                        t0 = time.time()
+                        if png is not None:
+                            video_io.write_frames(frame_dir, png, start=s)
+                        writer.write(video)
+                        write_time += time.time() - t0
+                torch.cuda.synchronize(device)
+            except BaseException:
+                if writer is not None and os.path.exists(video_path_out):
+                    os.remove(video_path_out)  # a partial mp4 would pass for a result
+                raise
+            run_time = time.time() - start - write_time  # GPU work and device-to-host copies, not file writing
             if rank != 0:
                 continue
-            video_path_out, frame_dir = output_paths(args, video_name)
-            if png is not None:
-                video_io.write_frames(frame_dir, png)
-            os.makedirs(os.path.dirname(video_path_out), exist_ok=True)
-            video_io.write_video(video_path_out, video, fps)
             written.append(video_path_out)
             log(f"{index_str} Saving upscaled video... time (sec): {run_time:.2f} \n")
         if written:

@@ -15,7 +15,7 @@ from __future__ import annotations
 
 import inspect
 from dataclasses import dataclass
-from typing import Any, List, Optional, Union
+from typing import Any, Iterator, List, Optional, Tuple, Union
 
 import torch
 
@@ -214,7 +214,29 @@ class VideoUpscalePipeline(ConfigMixin):
                  latents: Optional[torch.Tensor] = None, prompt_embeds: Optional[torch.Tensor] = None,
                  negative_prompt_embeds: Optional[torch.Tensor] = None, propagation_steps: list = [], w_lr: float = 1,
                  return_dict: bool = True, *, noise: Optional[torch.Tensor] = None):
-        """`noise` (keyword-only extension): the LR-noise draw of pipeline...:547, for generator-independent tests."""
+        """`noise` (keyword-only extension): the LR-noise draw of pipeline...:547, for generator-independent tests.
+        The whole clip: `sample_latents`, then every chunk of `decode_chunks` concatenated along time."""
+        sampled = self.sample_latents(prompt, image, flows_bi, num_inference_steps, guidance_scale, noise_level,
+                                      denoise_level, negative_prompt, num_images_per_prompt, eta, generator, latents,
+                                      prompt_embeds, negative_prompt_embeds, propagation_steps, w_lr, noise=noise)
+        frames = [f for _, _, f in self.decode_chunks(sampled)]
+        images = torch.cat(frames, dim=2) if len(frames) > 1 else frames[0]
+        if not return_dict:
+            return (images, sampled.latents)
+        return StableDiffusionPipelineOutput(images=images, nsfw_content_detected=None)
+
+    @torch.no_grad()
+    def sample_latents(self, prompt: Union[str, List[str]] = None, image: torch.Tensor = None,
+                       flows_bi: Optional[list] = None, num_inference_steps: int = 75, guidance_scale: float = 9.0,
+                       noise_level: int = 20, denoise_level: Optional[int] = None,
+                       negative_prompt: Optional[Union[str, List[str]]] = None, num_images_per_prompt: Optional[int] = 1,
+                       eta: float = 0.0, generator=None, latents: Optional[torch.Tensor] = None,
+                       prompt_embeds: Optional[torch.Tensor] = None, negative_prompt_embeds: Optional[torch.Tensor] = None,
+                       propagation_steps: list = [], w_lr: float = 1, *,
+                       noise: Optional[torch.Tensor] = None) -> "SampledLatents":
+        """`__call__` up to the decode (same arguments but `return_dict`): the denoised latents of the whole clip and
+        what the decoder needs with them.  `decode_chunks` turns the record into output frames a few at a time, so a
+        caller that consumes them chunk by chunk never holds the whole clip at output resolution."""
         self.check_inputs(prompt, image, noise_level, negative_prompt, prompt_embeds, negative_prompt_embeds)
         if image is None:
             raise ValueError("`image` input cannot be undefined.")
@@ -331,26 +353,38 @@ class VideoUpscalePipeline(ConfigMixin):
                 x0 = self.propagator(x0, ff, fb, interpolation="nearest", mode="fuse", fuse_scale=0.5, alpha1=0.001, alpha2=0.05)
             latents = self.scheduler.step_vt(x0, noise_pred, t, latents, **extra).prev_sample
 
-        # decode in 3-frame chunks (pipeline...:668-702); chunks are dealt round-robin to ranks
-        latents = latents.float()
-        latents_out = latents.clone()
+        return SampledLatents(latents=latents.float(), image_dec=image_dec, w_lr=w_lr)
+
+    @torch.no_grad()
+    def decode_chunks(self, sampled: "SampledLatents") -> Iterator[Tuple[int, int, torch.Tensor]]:
+        """Decode `sample_latents`' record in the reference's independent 3-frame chunks (pipeline...:668-702): yields
+        `(s, e, frames)` in time order, `frames` the clamped fp32 (b, 3, e - s, 4H, 4W) output of frames [s, e).
+        With several ranks, chunk k is decoded by rank k % world and each run of `world` consecutive chunks is
+        exchanged in one all_gather, so every rank yields every chunk and holds at most `world` of them at a time."""
+        latents, image_dec, w_lr = sampled.latents, sampled.image_dec, sampled.w_lr
+        rank, world = sharding.world_info(self.process_group)
+        b, _, T, H, W = latents.shape
         chunks = sharding.decode_chunks(T)
-        local = {}
-        for ci, (s, e) in enumerate(chunks):
-            if ci % world == rank:
+        shape = (b, self.vae.config.out_channels, sharding.DECODE_SEQ, 4 * H, 4 * W)
+        for g0 in range(0, len(chunks), world):
+            group = chunks[g0:g0 + world]  # chunk g0 + k belongs to rank k: g0 is a multiple of world
+            local = {}
+            if rank < len(group):
+                s, e = group[rank]
                 d = self.decode_latents_vsr(latents[:, :, s:e], image_dec[:, :, s:e], w_lr)
                 if e - s < sharding.DECODE_SEQ and world > 1:  # pad the ragged last chunk for the fixed-size gather
-                    pad = torch.zeros(d.shape[0], d.shape[1], sharding.DECODE_SEQ, *d.shape[3:], dtype=d.dtype, device=device)
+                    pad = torch.zeros(shape, dtype=d.dtype, device=d.device)
                     pad[:, :, : e - s] = d
                     d = pad
-                local[ci] = d
-        if world > 1:
-            shape = (latents.shape[0], self.vae.config.out_channels, sharding.DECODE_SEQ, 4 * H, 4 * W)
-            outs = sharding.all_gather_units(local, len(chunks), shape, torch.float32, device, self.process_group)
-            frames = [o[:, :, : e - s] for o, (s, e) in zip(outs, chunks)]
-        else:
-            frames = [local[ci] for ci in range(len(chunks))]
-        images = torch.cat(frames, dim=2) if len(frames) > 1 else frames[0]
-        if not return_dict:
-            return (images, latents_out)
-        return StableDiffusionPipelineOutput(images=images, nsfw_content_detected=None)
+                local[rank] = d
+            outs = sharding.all_gather_units(local, len(group), shape, torch.float32, latents.device, self.process_group)
+            for (s, e), o in zip(group, outs):
+                yield s, e, o[:, :, : e - s]
+
+
+@dataclass
+class SampledLatents:
+    """What `VideoUpscalePipeline.sample_latents` hands to `decode_chunks`."""
+    latents: torch.Tensor    # (b, 4, T, H, W) fp32 denoised latents
+    image_dec: torch.Tensor  # (b, 3, T, H, W) fp32 LR frames that condition the decoder
+    w_lr: float

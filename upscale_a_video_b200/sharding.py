@@ -6,7 +6,7 @@ step_v0, flow propagation — a recurrence over the WHOLE clip — and step_vt) 
 So: one process per GPU with replicated weights, window w of the step goes to rank `w % world`, ONE all_gather of
 the windows' noise predictions per step (the "propagation boundary"), after which every rank redundantly runs
 the elementwise tail in the reference's exact window order (the 0.5/0.5 blend is order dependent).  Decode chunks
-are dealt the same way and gathered once at the end.  No collective exists when world == 1.
+are dealt the same way and gathered `world` at a time.  No collective exists when world == 1.
 """
 from __future__ import annotations
 

@@ -4,16 +4,18 @@ plan + executor, so that large frames can be dealt to GPUs tile by tile.
 `plan_tiles` reproduces the reference geometry exactly (tiles of `tile_size` plus `overlap` LR pixels of context on every
 side, the last row / column merged into its neighbour when the remainder is <= overlap, hard paste of the central region,
 no blending); it is pinned by `tests/golden/tiles.json`, which is produced by EXECUTING the reference's own loop
-(`oracle/make_golden_tiles.py`).  `upscale_tiled` runs the pipeline per tile.  With torch.distributed initialised, tiles are
-dealt round-robin to ranks (each tile is an independent pipeline run: no per-step collective at all) and the pasted outputs
-are combined with one all_reduce at the end.  The reference consumes ONE generator sequentially over the tiles
-(inference...:197,268); to keep that stream every rank draws the noise of every tile in loop order and uses its own.
+(`oracle/make_golden_tiles.py`).  `upscale_tiled` runs the pipeline per tile; `iter_upscale_tiled` samples every tile
+first, then decodes and pastes 3 frames at a time, so that the output never exists for the whole clip at once.  With
+torch.distributed initialised, tiles are dealt round-robin to ranks (each tile is an independent pipeline run: no per-step
+collective at all) and the pasted outputs are combined with one all_reduce, at the end or per chunk.  The reference
+consumes ONE generator sequentially over the tiles (inference...:197,268); to keep that stream every rank draws the noise
+of every tile in loop order and uses its own.
 """
 from __future__ import annotations
 
 import math
 from dataclasses import dataclass
-from typing import List, Optional, Tuple
+from typing import Iterator, List, Optional, Tuple
 
 import torch
 
@@ -71,15 +73,12 @@ def _solo_group(rank: int, world: int):
     return _SOLO_GROUPS[world][rank]
 
 
-@torch.no_grad()
-def upscale_tiled(pipeline, image: torch.Tensor, flows_bi: Optional[list] = None, generator=None, tile_size: int = 256,
-                  overlap: int = 64, process_group=None, **pipe_kwargs) -> torch.Tensor:
-    """image: (1, 3, T, H, W) LR clip in [-1, 1] on the GPU.  Returns the (1, 3, T, 4H, 4W) output like the reference's
-    tile branch.  `pipe_kwargs` go to `VideoUpscalePipeline.__call__` (prompt / prompt_embeds, steps, guidance, ...)."""
-    b, c, t, h, w = image.shape
-    plan = plan_tiles(h, w, tile_size, overlap)
+def _rank_tiles(pipeline, image, flows_bi, generator, plan, process_group, pipe_kwargs):
+    """Yields `(tile, LR clip of the tile, its flows, noise, initial latents)` for this rank's tiles in plan order, while
+    `pipeline.process_group` is this rank's single-rank group.  Every rank draws every tile's noise from the one
+    generator, so each tile gets the draw the reference's serial loop would give it."""
+    b, _, t, _, _ = image.shape
     rank, world = sharding.world_info(process_group)
-    out = image.new_zeros((b, c, t, 4 * h, 4 * w), dtype=torch.float32)
     dtype = None
     for key in ("prompt_embeds", "negative_prompt_embeds"):
         if pipe_kwargs.get(key) is not None:
@@ -89,11 +88,8 @@ def upscale_tiled(pipeline, image: torch.Tensor, flows_bi: Optional[list] = None
     c_lat = pipeline.vae.config.latent_channels
     # tiles are independent pipeline runs: inside a tile the pipeline must not shard windows over the same ranks
     saved_group = pipeline.process_group
-    solo = None
-    if world > 1:
-        solo = _solo_group(rank, world)
     try:
-        pipeline.process_group = solo if world > 1 else saved_group
+        pipeline.process_group = _solo_group(rank, world) if world > 1 else saved_group
         for i, tl in enumerate(plan):
             py0, py1, px0, px1 = tl.in_box
             tile = image[:, :, :, py0:py1, px0:px1]
@@ -105,13 +101,58 @@ def upscale_tiled(pipeline, image: torch.Tensor, flows_bi: Optional[list] = None
             flows = None
             if flows_bi is not None:
                 flows = [f[:, :, :, py0:py1, px0:px1] for f in flows_bi]
-            res = pipeline(image=tile, flows_bi=flows, noise=noise, latents=latents, **pipe_kwargs).images
-            oy0, oy1, ox0, ox1 = tl.out_box
-            sy0, sy1, sx0, sx1 = tl.src_box
-            out[:, :, :, oy0:oy1, ox0:ox1] = res[:, :, :, sy0:sy1, sx0:sx1]
+            yield tl, tile, flows, noise, latents
     finally:
         pipeline.process_group = saved_group
-    if world > 1:
+
+
+def _paste(out, tl, res):
+    oy0, oy1, ox0, ox1 = tl.out_box
+    sy0, sy1, sx0, sx1 = tl.src_box
+    out[:, :, :, oy0:oy1, ox0:ox1] = res[:, :, :, sy0:sy1, sx0:sx1]
+
+
+@torch.no_grad()
+def upscale_tiled(pipeline, image: torch.Tensor, flows_bi: Optional[list] = None, generator=None, tile_size: int = 256,
+                  overlap: int = 64, process_group=None, **pipe_kwargs) -> torch.Tensor:
+    """image: (1, 3, T, H, W) LR clip in [-1, 1] on the GPU.  Returns the (1, 3, T, 4H, 4W) output like the reference's
+    tile branch.  `pipe_kwargs` go to `VideoUpscalePipeline.__call__` (prompt / prompt_embeds, steps, guidance, ...)."""
+    b, c, t, h, w = image.shape
+    plan = plan_tiles(h, w, tile_size, overlap)
+    out = image.new_zeros((b, c, t, 4 * h, 4 * w), dtype=torch.float32)
+    for tl, tile, flows, noise, latents in _rank_tiles(pipeline, image, flows_bi, generator, plan, process_group,
+                                                       pipe_kwargs):
+        _paste(out, tl, pipeline(image=tile, flows_bi=flows, noise=noise, latents=latents, **pipe_kwargs).images)
+    if sharding.world_info(process_group)[1] > 1:
         import torch.distributed as dist
         dist.all_reduce(out, group=process_group)  # paste regions are disjoint: sum == union
     return out
+
+
+@torch.no_grad()
+def iter_upscale_tiled(pipeline, image: torch.Tensor, flows_bi: Optional[list] = None, generator=None,
+                       tile_size: int = 256, overlap: int = 64, process_group=None,
+                       **pipe_kwargs) -> Iterator[Tuple[int, int, torch.Tensor]]:
+    """`upscale_tiled` a few frames at a time: yields `(s, e, chunk)` in the order of `sharding.decode_chunks(T)`, `chunk`
+    the fp32 (1, 3, e - s, 4H, 4W) output of frames [s, e), equal to `upscale_tiled(...)[:, :, s:e]`.  Every tile of
+    this rank is sampled first (`pipeline.sample_latents`) and only its latents are kept; then each chunk decodes every
+    tile's frames [s, e) (`pipeline.decode_latents_vsr`) and pastes them, with one all_reduce per chunk across ranks."""
+    b, c, t, h, w = image.shape
+    plan = plan_tiles(h, w, tile_size, overlap)
+    sampled = []
+    for tl, tile, flows, noise, latents in _rank_tiles(pipeline, image, flows_bi, generator, plan, process_group,
+                                                       pipe_kwargs):
+        r = pipeline.sample_latents(image=tile, flows_bi=flows, noise=noise, latents=latents, **pipe_kwargs)
+        sampled.append((tl, r.latents, r.w_lr))
+        del r  # the record's LR copy is taken again from `image` per chunk
+    world = sharding.world_info(process_group)[1]
+    for s, e in sharding.decode_chunks(t):
+        out = image.new_zeros((b, c, e - s, 4 * h, 4 * w), dtype=torch.float32)
+        for tl, latents, w_lr in sampled:
+            py0, py1, px0, px1 = tl.in_box
+            lr = image[:, :, s:e, py0:py1, px0:px1].to(torch.float32)
+            _paste(out, tl, pipeline.decode_latents_vsr(latents[:, :, s:e], lr, w_lr))
+        if world > 1:
+            import torch.distributed as dist
+            dist.all_reduce(out, group=process_group)  # paste regions are disjoint: sum == union
+        yield s, e, out

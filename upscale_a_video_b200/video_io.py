@@ -95,27 +95,46 @@ def read_frames(path: str) -> Tuple[np.ndarray, Optional[float], str]:
     return np.stack(frames), fps, name
 
 
+class VideoWriter:
+    """mp4 (fourcc mp4v) written chunk by chunk: opened once for frames of (h, w), then `write((t, h, w, 3) uint8 RGB)`
+    per chunk; fps None -> DEFAULT_FPS.  A context manager: the file is finalised when the block ends."""
+
+    def __init__(self, path: str, fps: Optional[float], size: Tuple[int, int]):
+        cv2 = _cv2()
+        self.path, self.size = path, tuple(size)
+        h, w = self.size
+        self._writer = cv2.VideoWriter(path, cv2.VideoWriter_fourcc(*"mp4v"), float(fps or DEFAULT_FPS), (w, h))
+        if not self._writer.isOpened():
+            raise RuntimeError(f"OpenCV cannot write the video {path}")
+
+    def write(self, frames_rgb: np.ndarray) -> None:
+        t, h, w, c = frames_rgb.shape
+        assert c == 3 and frames_rgb.dtype == np.uint8 and (h, w) == self.size
+        for frame in frames_rgb:
+            self._writer.write(np.ascontiguousarray(frame[..., ::-1]))
+
+    def close(self) -> None:
+        self._writer.release()
+
+    def __enter__(self) -> "VideoWriter":
+        return self
+
+    def __exit__(self, *exc) -> None:
+        self.close()
+
+
 def write_video(path: str, frames_rgb: np.ndarray, fps: Optional[float]) -> None:
     """mp4 (fourcc mp4v) of (t, h, w, 3) uint8 RGB frames; fps None -> DEFAULT_FPS"""
-    cv2 = _cv2()
-    t, h, w, c = frames_rgb.shape
-    assert c == 3 and frames_rgb.dtype == np.uint8
-    writer = cv2.VideoWriter(path, cv2.VideoWriter_fourcc(*"mp4v"), float(fps or DEFAULT_FPS), (w, h))
-    if not writer.isOpened():
-        raise RuntimeError(f"OpenCV cannot write the video {path}")
-    try:
-        for frame in frames_rgb:
-            writer.write(np.ascontiguousarray(frame[..., ::-1]))
-    finally:
-        writer.release()
+    with VideoWriter(path, fps, frames_rgb.shape[1:3]) as writer:
+        writer.write(frames_rgb)
 
 
-def write_frames(folder: str, frames_rgb: np.ndarray) -> List[str]:
-    """one PNG per frame of (t, h, w, 3) uint8 RGB frames: folder/0000.png, folder/0001.png, ..."""
+def write_frames(folder: str, frames_rgb: np.ndarray, start: int = 0) -> List[str]:
+    """one PNG per frame of (t, h, w, 3) uint8 RGB frames, numbered from `start`: folder/0000.png, folder/0001.png, ..."""
     cv2 = _cv2()
     os.makedirs(folder, exist_ok=True)
     paths = []
-    for i, frame in enumerate(frames_rgb):
+    for i, frame in enumerate(frames_rgb, start):
         p = os.path.join(folder, f"{i:04d}.png")
         if not cv2.imwrite(p, np.ascontiguousarray(frame[..., ::-1])):
             raise RuntimeError(f"OpenCV cannot write {p}")
