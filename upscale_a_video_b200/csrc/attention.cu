@@ -723,6 +723,9 @@ uav_status_t uav_attention(const void* q, const void* k, const void* v, void* ou
   }
   UAV_REQUIRE(head_dim != 512 || heads == 1, "uav_attention: head_dim 512 supports a single head");
   UAV_REQUIRE(nq <= INT32_MAX && nk <= INT32_MAX, "uav_attention: nq or nk too large");
+  // the cross and wgmma kernels take the row maximum of the raw scores and scale it afterwards, which is the maximum of
+  // the scaled scores only for scale > 0 (scale = 0 would also turn the masked columns into -inf * 0 = NaN)
+  UAV_REQUIRE(scale > 0.f && scale < INFINITY, "uav_attention: scale must be finite and > 0 (got %g)", (double)scale);
   UAV_REQUIRE_ALIGNED16("uav_attention", q);
   UAV_REQUIRE_ALIGNED16("uav_attention", k);
   UAV_REQUIRE_ALIGNED16("uav_attention", v);

@@ -441,7 +441,9 @@ def layer_norm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: fl
 # attention
 # ------------------------------------------------------------------------------------------------
 def attention(q, k, v, heads: int, *, kv_batch_div: int = 1, scale: Optional[float] = None, out=None):
-    """q: (batch, nq, heads*d) fp16 (may be a column slice of a fused qkv buffer); k, v: (batch/kv_batch_div, nk, heads*d)."""
+    """q: (batch, nq, heads*d) fp16 (may be a column slice of a fused qkv buffer); k, v: (batch/kv_batch_div, nk, heads*d).
+    `scale` (default d ** -0.5) multiplies the scores before the softmax; it must be finite and > 0, anything else is
+    rejected before a launch."""
     batch, nq, C = q.shape
     d = C // heads
     nk = k.shape[1]
