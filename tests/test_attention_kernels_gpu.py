@@ -93,19 +93,19 @@ def run_attention(q, k, v, heads, kvd, scale=None):
 
 # ---------------------------------------------------------------- dispatch boundaries
 # (B, heads, d, nq, nk, kv_batch_div, kernel).  uav_attention runs the cross kernel (80- or 128-key resident tile) for
-# nk <= 128, nq >= 4 nk and d != 512, the wgmma kernel for the other d = 128 / 512 cases (128- and 64-key tiles, 128 query
-# rows per CTA) and flash_attn_kernel (64-key tiles, 64 query rows) for the other d = 64 cases.
+# nk <= 128, nq >= 4 nk and d != 512, and the wgmma kernel for every other case (128 query rows per CTA; 128-key tiles
+# for d = 64 and 128, 64-key tiles for d = 512).
 CROSS64_5, CROSS64_8 = "cross_attn_kernel<64,5>", "cross_attn_kernel<64,8>"
 CROSS128_5, CROSS128_8 = "cross_attn_kernel<128,5>", "cross_attn_kernel<128,8>"
-FLASH, TC128, TC512 = "flash_attn_kernel", "fa_tc_kernel<128,128,128>", "fa_tc_kernel<512,256,64>"
+TC64, TC128, TC512 = "fa_tc_kernel<64,64,128>", "fa_tc_kernel<128,128,128>", "fa_tc_kernel<512,256,64>"
 DISPATCH = [
-    (2, 8, 64, 4, 1, 1, CROSS64_5), (2, 8, 64, 3, 1, 1, FLASH),
-    (4, 8, 64, 64, 16, 2, CROSS64_5), (4, 8, 64, 63, 16, 2, FLASH),
-    (8, 8, 64, 308, 77, 8, CROSS64_5), (8, 8, 64, 307, 77, 8, FLASH),
-    (2, 8, 64, 320, 80, 1, CROSS64_5), (2, 8, 64, 324, 81, 1, CROSS64_8), (2, 8, 64, 323, 81, 1, FLASH),
-    (2, 8, 64, 508, 127, 2, CROSS64_8), (2, 8, 64, 512, 128, 1, CROSS64_8), (2, 8, 64, 511, 128, 1, FLASH),
-    (2, 8, 64, 516, 129, 1, FLASH), (2, 4, 64, 129, 191, 1, FLASH), (2, 4, 64, 127, 192, 1, FLASH),
-    (2, 4, 64, 193, 193, 1, FLASH), (8, 2, 64, 65, 257, 8, FLASH),
+    (2, 8, 64, 4, 1, 1, CROSS64_5), (2, 8, 64, 3, 1, 1, TC64),
+    (4, 8, 64, 64, 16, 2, CROSS64_5), (4, 8, 64, 63, 16, 2, TC64),
+    (8, 8, 64, 308, 77, 8, CROSS64_5), (8, 8, 64, 307, 77, 8, TC64),
+    (2, 8, 64, 320, 80, 1, CROSS64_5), (2, 8, 64, 324, 81, 1, CROSS64_8), (2, 8, 64, 323, 81, 1, TC64),
+    (2, 8, 64, 508, 127, 2, CROSS64_8), (2, 8, 64, 512, 128, 1, CROSS64_8), (2, 8, 64, 511, 128, 1, TC64),
+    (2, 8, 64, 516, 129, 1, TC64), (2, 4, 64, 129, 191, 1, TC64), (2, 4, 64, 127, 192, 1, TC64),
+    (2, 4, 64, 193, 193, 1, TC64), (8, 2, 64, 65, 257, 8, TC64),
     (8, 8, 128, 308, 77, 8, CROSS128_5), (2, 8, 128, 324, 81, 1, CROSS128_8), (2, 8, 128, 512, 128, 2, CROSS128_8),
     (2, 8, 128, 511, 128, 2, TC128), (2, 8, 128, 516, 129, 1, TC128), (2, 8, 128, 307, 77, 1, TC128),
     (2, 4, 128, 256, 255, 1, TC128), (2, 4, 128, 129, 256, 1, TC128), (8, 2, 128, 127, 257, 8, TC128),
@@ -113,7 +113,7 @@ DISPATCH = [
     (2, 1, 512, 256, 64, 1, TC512), (2, 1, 512, 127, 65, 1, TC512), (2, 1, 512, 385, 129, 2, TC512),
     (1, 1, 512, 300, 191, 1, TC512),
 ]
-ATTENTION_KERNELS = {CROSS64_5, CROSS64_8, CROSS128_5, CROSS128_8, FLASH, TC128, TC512}
+ATTENTION_KERNELS = {CROSS64_5, CROSS64_8, CROSS128_5, CROSS128_8, TC64, TC128, TC512}
 
 
 def _id(c):
@@ -135,7 +135,7 @@ def dispatched(uav_lib):
     return _in_subprocess("dispatch_kernels")
 
 
-@pytest.mark.parametrize("case", DISPATCH, ids=_id)
+@pytest.mark.parametrize("case", DISPATCH, ids=lambda c: f"{_id(c)}-{c[6]}")  # the id names the kernel it pins
 def test_dispatch_boundaries(case, dispatched):
     """each case runs the kernel of its row (and no other attention kernel), passes the criterion on every generator,
     keeps its operands' NaN surroundings out and its output sentinel intact, and repeats bit for bit"""

@@ -12,12 +12,18 @@ def timeit(fn, iters=3, warmup=1):
     for _ in range(iters): fn()
     e.record(); torch.cuda.synchronize()
     return s.elapsed_time(e) / iters
-for name, B, heads, d, n in [("vae d512 N=46080", 1, 1, 512, 46080), ("vae d512 N=184320", 1, 1, 512, 184320),
-                             ("unet self d128 N=2880 x16 frames", 16, 8, 128, 2880)]:
+# the d = 64 self-attention rows are no pipeline shape (the UNet's d = 64 attention is text cross-attention): they time
+# the d = 64 instance of the wgmma kernel that d = 128 runs on
+for name, B, heads, d, n, iters in [("vae d512 N=46080", 1, 1, 512, 46080, 3),
+                                    ("vae d512 N=184320", 1, 1, 512, 184320, 3),
+                                    ("unet self d128 N=2880 x16 frames", 16, 8, 128, 2880, 3),
+                                    ("self d64 N=920 x16", 16, 8, 64, 920, 200),
+                                    ("self d64 N=2880 x16", 16, 8, 64, 2880, 50),
+                                    ("self d64 N=14400 x16", 16, 8, 64, 14400, 10)]:
     C = heads * d
     qkv = torch.randn(B, n, 3 * C, device="cuda").half()
     out = torch.empty(B, n, C, device="cuda", dtype=torch.float16)
-    ms = timeit(lambda: ops.attention(qkv[..., :C], qkv[..., C:2*C], qkv[..., 2*C:], heads, out=out))
+    ms = timeit(lambda: ops.attention(qkv[..., :C], qkv[..., C:2*C], qkv[..., 2*C:], heads, out=out), iters=iters)
     print(json.dumps({"name": name, "ms": ms, "tflops_alg": 4.0 * B * n * n * C / ms / 1e9}))
 
 # temporal attention at the top UNet level (B=2, T=8, 160x288, 8 heads x 64): 8 B/element stream

@@ -3,10 +3,9 @@
 //  * uav_attention: softmax(Q K^T * scale) V without materialising the score matrix
 //    (the reference materialises it: attention.py:209-238, 2.1 GB per call at 320x576).
 //    Short key sequences (the text cross-attention: Nk = 77, d = 64/128, K/V shared by all
-//    frames of a batch item) run on a resident-KV mma.sync kernel.  Otherwise d = 128 (UNet
-//    spatial self-attention, N = h*w) and d = 512 (VAE mid-block attention, 1 head) run on the
-//    wgmma kernel of attention_tc.cu, and d = 64 on a FlashAttention-2 style mma.sync.m16n8k16
-//    kernel (fp16 in, fp32 accumulate, fp32 online softmax).
+//    frames of a batch item) run on a resident-KV mma.sync kernel.  Every other case (UNet
+//    spatial self-attention, d = 128, N = h*w; VAE mid-block attention, d = 512, 1 head; and
+//    d = 64 off the pipeline's shapes) runs on the wgmma kernel of attention_tc.cu.
 //  * uav_temporal_attention: the seq = T per-pixel attention with rotary embedding on the
 //    first 32 dims and the T5-style relative-position bias (attention.py:699-733).  T <= 8 (the
 //    pipeline's windows) with an even head count runs on an mma.sync kernel for a pair of heads;
@@ -14,7 +13,7 @@
 //    16-frame key tiles.  Both read q/k/v in the (b, f, hw, c) layout, so the reference's two
 //    "(b f) d c <-> (b d) f c" rearrange copies (attention.py:555,560) do not exist.
 //
-// All four kernels are built from the warp-tile helpers below: S = Q K^T, the P fragment, O += P V and the output
+// All three kernels are built from the warp-tile helpers below: S = Q K^T, the P fragment, O += P V and the output
 // staging are written once.
 #include "uav_common.cuh"
 
@@ -87,12 +86,7 @@ __device__ __forceinline__ void stage_rows(__half* tile, int r0, const float (&o
   }
 }
 
-// ---------------------------------------------------------------------------------------
-// flash attention (mma.sync), d = 64
-// ---------------------------------------------------------------------------------------
 constexpr int FA_BM = 64;   // query rows per CTA (4 warps x 16)
-constexpr int FA_BN = 64;   // kv rows per iteration
-constexpr int FA_D = 64;    // head dim
 constexpr int FA_THREADS = 128;
 
 struct FaParams {
@@ -106,143 +100,13 @@ struct FaParams {
   float scale_log2;                  // softmax scale * log2(e)
 };
 
-__global__ void __launch_bounds__(FA_THREADS)
-    flash_attn_kernel(const FaParams p) {
-  extern __shared__ __align__(16) uint8_t fa_smem[];
-  __half* sq = reinterpret_cast<__half*>(fa_smem);  // [64][FA_D]
-  __half* sk = sq + FA_BM * FA_D;                   // [2][64][FA_D]
-  __half* sv = sk + 2 * FA_BN * FA_D;               // [2][64][FA_D]
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int bh = blockIdx.y;
-  const int b = bh / p.heads, h = bh % p.heads;
-  const int q0 = blockIdx.x * FA_BM;
-  const __half* qg = p.q + b * p.bsq + static_cast<int64_t>(h) * FA_D;
-  const __half* kg = p.k + (b / p.kv_batch_div) * p.bsk + static_cast<int64_t>(h) * FA_D;
-  const __half* vg = p.v + (b / p.kv_batch_div) * p.bsv + static_cast<int64_t>(h) * FA_D;
-  __half* og = p.o + b * p.bso + static_cast<int64_t>(h) * FA_D;
-
-  constexpr int QC = FA_D / 8;  // 16B chunks per row
-  // ---- async loads: Q tile, then K/V tile 0 ----
-  for (int i = tid; i < FA_BM * QC; i += FA_THREADS) {
-    const int r = i / QC, c = i % QC;
-    const bool ok = q0 + r < p.nq;
-    cp_async16(tile_ptr<FA_D>(sq, r, c), qg + static_cast<int64_t>(ok ? q0 + r : 0) * p.ldq + c * 8,
-               ok);
-  }
-  auto load_kv = [&](int tile, int buf) {
-    const int k0 = tile * FA_BN;
-    __half* skb = sk + buf * FA_BN * FA_D;
-    __half* svb = sv + buf * FA_BN * FA_D;
-    for (int i = tid; i < FA_BN * QC; i += FA_THREADS) {
-      const int r = i / QC, c = i % QC;
-      const bool ok = k0 + r < p.nk;
-      cp_async16(tile_ptr<FA_D>(skb, r, c),
-                 kg + static_cast<int64_t>(ok ? k0 + r : 0) * p.ldk + c * 8, ok);
-    }
-    for (int i = tid; i < FA_BN * QC; i += FA_THREADS) {
-      const int r = i / QC, c = i % QC;
-      const bool ok = k0 + r < p.nk;
-      cp_async16(tile_ptr<FA_D>(svb, r, c),
-                 vg + static_cast<int64_t>(ok ? k0 + r : 0) * p.ldv + c * 8, ok);
-    }
-  };
-  load_kv(0, 0);
-  cp_async_commit();
-
-  const int ntiles = (p.nk + FA_BN - 1) / FA_BN;
-  float o_acc[FA_D / 8][4];
-#pragma unroll
-  for (int i = 0; i < FA_D / 8; ++i) o_acc[i][0] = o_acc[i][1] = o_acc[i][2] = o_acc[i][3] = 0.f;
-  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
-
-  const int g = lane >> 2, t4 = lane & 3;
-  const int arow = warp * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;  // ldmatrix A row
-  for (int tile = 0; tile < ntiles; ++tile) {
-    const int buf = tile & 1;
-    if (tile + 1 < ntiles) load_kv(tile + 1, buf ^ 1);
-    cp_async_commit();
-    cp_async_wait<1>();
-    __syncthreads();
-    __half* skb = sk + buf * FA_BN * FA_D;
-    __half* svb = sv + buf * FA_BN * FA_D;
-
-    // ---- S = Q K^T (16 x 64 per warp) ----
-    float s[FA_BN / 8][4];
-#pragma unroll
-    for (int i = 0; i < FA_BN / 8; ++i) s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f;
-    warp_qk<FA_D, FA_BN / 16>(s, sq, arow, skb, lane);
-    // ---- mask + online softmax (rows g and g+8 of this warp's 16) ----
-    const int kbase = tile * FA_BN;
-    float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-    for (int nb = 0; nb < FA_BN / 8; ++nb) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int col = kbase + nb * 8 + t4 * 2 + (e & 1);
-        float x = s[nb][e] * p.scale_log2;
-        if (col >= p.nk) x = -INFINITY;
-        s[nb][e] = x;
-        mx[e >> 1] = fmaxf(mx[e >> 1], x);
-      }
-    }
-#pragma unroll
-    for (int r = 0; r < 2; ++r) mx[r] = quad_max(mx[r]);
-    float corr[2], rs[2] = {0.f, 0.f};
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      const float mnew = fmaxf(m_run[r], mx[r]);
-      corr[r] = (m_run[r] == -INFINITY) ? 0.f : exp2f(m_run[r] - mnew);
-      m_run[r] = mnew;
-    }
-    uint32_t pf[FA_BN / 16][4];  // P as the A fragments of the k16 steps
-#pragma unroll
-    for (int nb = 0; nb < FA_BN / 8; ++nb) {
-      const float p0 = exp2f(s[nb][0] - m_run[0]), p1 = exp2f(s[nb][1] - m_run[0]);
-      const float p2 = exp2f(s[nb][2] - m_run[1]), p3 = exp2f(s[nb][3] - m_run[1]);
-      rs[0] += p0 + p1;
-      rs[1] += p2 + p3;
-      pack_p(pf[nb >> 1], nb & 1, p0, p1, p2, p3);
-    }
-#pragma unroll
-    for (int r = 0; r < 2; ++r) l_run[r] = l_run[r] * corr[r] + rs[r];
-#pragma unroll
-    for (int i = 0; i < FA_D / 8; ++i) {
-      o_acc[i][0] *= corr[0];
-      o_acc[i][1] *= corr[0];
-      o_acc[i][2] *= corr[1];
-      o_acc[i][3] *= corr[1];
-    }
-    // ---- O += P V ----
-#pragma unroll
-    for (int kk = 0; kk < FA_BN / 16; ++kk) warp_pv<FA_D>(o_acc, pf[kk], svb, kk * 16, lane);
-    __syncthreads();  // all warps done with buf before it is refilled
-  }
-  cp_async_wait<0>();
-
-  // ---- finalize: O / l -> smem (reuse Q tile region) -> coalesced stores ----
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const float l = quad_sum(l_run[r]);
-    l_run[r] = (l > 0.f) ? 1.f / l : 0.f;
-  }
-  __half* so = sq;  // [64][FA_D]
-  stage_rows<FA_D>(so, warp * 16 + g, o_acc, l_run[0], l_run[1], t4);
-  __syncthreads();
-  for (int i = tid; i < FA_BM * QC; i += FA_THREADS) {
-    const int r = i / QC, c = i % QC;
-    if (q0 + r < p.nq)
-      stg16(og + static_cast<int64_t>(q0 + r) * p.ldo + c * 8,
-            *reinterpret_cast<const uint4*>(tile_ptr<FA_D>(so, r, c)));
-  }
-}
-
 // ---------------------------------------------------------------------------------------
 // text cross-attention (nk <= 128, typically 77): K and V of one (batch, head) stay resident in
 // shared memory, the CTA streams query tiles past them (double-buffered cp.async), the whole
 // score row fits in registers (single-pass softmax), and each warp stages its 16 output rows in
-// the Q buffer it has just consumed.  The generic kernel above spends most of its time in the
-// per-CTA prologue / epilogue when there are only two KV tiles (measured 1.0 TB/s at h/2).
+// the Q buffer it has just consumed.  A kernel that streams KV tiles past one query tile per CTA
+// spends most of its time in the per-CTA prologue / epilogue when there are only one or two KV
+// tiles (an mma.sync one with 64-key tiles measured 1.0 TB/s at h/2).
 // ---------------------------------------------------------------------------------------
 template <int D, int NB16>
 __global__ void __launch_bounds__(FA_THREADS)
@@ -731,10 +595,10 @@ uav_status_t uav_attention(const void* q, const void* k, const void* v, void* ou
   UAV_REQUIRE_ALIGNED16("uav_attention", v);
   UAV_REQUIRE_ALIGNED16("uav_attention", out);
 
-  // short key/value sequences (the 77 prompt tokens) run on the resident-KV streaming kernel; otherwise d = 128 (UNet
-  // self-attention at h/8) and d = 512 (VAE AttentionBlock) run on the wgmma kernel and d = 64 on flash_attn_kernel
+  // short key/value sequences (the 77 prompt tokens) run on the resident-KV streaming kernel; everything else (UNet
+  // self-attention at h/8, d = 128; VAE AttentionBlock, d = 512; d = 64 off the pipeline's shapes) on the wgmma kernel
   const bool cross = nk <= 128 && nq >= 4 * nk && head_dim != 512;
-  if (!cross && head_dim != 64)
+  if (!cross)
     return attention_tc(q, k, v, out, batch, heads, head_dim, nq, nk, ldq, ldk, ldv, ldo, kv_batch_div, scale,
                         stream);
   FaParams p;
@@ -743,12 +607,8 @@ uav_status_t uav_attention(const void* q, const void* k, const void* v, void* ou
   p.bsq = nq * ldq; p.bsk = nk * ldk; p.bsv = nk * ldv; p.bso = nq * ldo;
   p.nq = (int)nq; p.nk = (int)nk; p.heads = heads; p.kv_batch_div = (int)kv_batch_div;
   p.scale_log2 = scale * 1.4426950408889634f;
-  if (cross) {
-    if (head_dim == 64) return nk <= 80 ? launch_cross<64, 5>(p, (int)batch, stream) : launch_cross<64, 8>(p, (int)batch, stream);
-    return nk <= 80 ? launch_cross<128, 5>(p, (int)batch, stream) : launch_cross<128, 8>(p, (int)batch, stream);
-  }
-  return launch_opted_in<flash_attn_kernel>(dim3((p.nq + FA_BM - 1) / FA_BM, batch * heads), FA_THREADS,
-                                            (FA_BM + 4 * FA_BN) * FA_D * 2, stream, p);
+  if (head_dim == 64) return nk <= 80 ? launch_cross<64, 5>(p, (int)batch, stream) : launch_cross<64, 8>(p, (int)batch, stream);
+  return nk <= 80 ? launch_cross<128, 5>(p, (int)batch, stream) : launch_cross<128, 8>(p, (int)batch, stream);
 }
 
 uav_status_t uav_temporal_attention(const void* q, const void* k, const void* v, void* out,

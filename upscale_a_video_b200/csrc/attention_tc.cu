@@ -1,8 +1,10 @@
 // attention_tc.cu — wgmma FlashAttention forward for the two dense attention cores of
 // the sampling path (SURVEY.md §8a rows a9, a19):
 //   * VAE mid-block AttentionBlock: 1 head, d = 512, N = h*w tokens per frame (184 320 at
-//     320x576 -> 70 TFLOP per frame, 71 % of VAE-decode FLOPs);
-//   * UNet spatial self-attention: 8 heads, d = 128, N = 2880.
+//     320x576 -> 70 TFLOP per frame, 71 % of VAE-decode FLOPs): fa_tc_kernel<512, 256, 64>;
+//   * UNet spatial self-attention: 8 heads, d = 128, N = 2880: fa_tc_kernel<128, 128, 128>.
+// d = 64 (no pipeline shape: the UNet's d = 64 attention is text cross-attention, attention.cu) runs on
+// fa_tc_kernel<64, 64, 128>.
 //
 // One CTA = 128 query rows x DVT output columns; warpgroup 0 is the TMA producer (one thread), warpgroups 1 and 2 each
 // own 64 query rows.  Per kv tile of BN rows a consumer warpgroup computes S = Q K^T with wgmma from shared memory
@@ -221,7 +223,8 @@ static uav_status_t launch_fa_tc(FaTcParams& p, int64_t batch, int dv_splits, cu
 }
 
 
-// entry used by uav_attention (attention.cu), which has validated the arguments, for head_dim 128 and 512 (one head)
+// entry used by uav_attention (attention.cu), which has validated the arguments, for head_dim 64, 128 and 512 (one
+// head)
 uav_status_t attention_tc(const void* q, const void* k, const void* v, void* out, int64_t batch,
                           int heads, int head_dim, int64_t nq, int64_t nk, int64_t ldq, int64_t ldk,
                           int64_t ldv, int64_t ldo, int64_t kv_batch_div, float scale,
@@ -252,6 +255,7 @@ uav_status_t attention_tc(const void* q, const void* k, const void* v, void* out
   p.kv_batch_div = (int)kv_batch_div;
   p.scale_log2 = scale * 1.4426950408889634f;
   if (head_dim == 512) return launch_fa_tc<512, 256, 64>(p, batch, 2, stream);
+  if (head_dim == 64) return launch_fa_tc<64, 64, 128>(p, batch, 1, stream);
   return launch_fa_tc<128, 128, 128>(p, batch, 1, stream);
 }
 
