@@ -411,10 +411,45 @@ uav_status_t uav_raft_convex_upsample(const float* coords1, const void* mask, in
 /* ---- CLIP text encoder (SURVEY.md §8f rank 3) ---------------------------------------------------------------
  * causal self-attention over a short sequence (transformers CLIPAttention under CLIPTextTransformer's causal mask):
  * q, k, v, out fp16 [batch][n][ld] with `heads * head_dim` used columns (column slices of a fused qkv buffer allowed),
- * n <= 128, head_dim <= 128 and even; out[i] = softmax_j<=i(scale * q_i . k_j) v_j */
+ * n <= 128, head_dim <= 128 and even; out[i] = softmax_j<=i(scale * q_i . k_j) v_j.  head_dim 128 also takes n > 128 (the
+ * LLaVA decoder's prefill) on the causal wgmma kernel: then token strides are multiples of 8, pointers 16-byte
+ * aligned and scale finite and > 0 */
 uav_status_t uav_attention_causal(const void* q, const void* k, const void* v, void* out, int64_t batch, int heads, int head_dim,
                                   int64_t n, int64_t ldq, int64_t ldk, int64_t ldv, int64_t ldo, float scale,
                                   uav_stream_t stream);
+
+/* ---- LLaVA-1.5 captioner (llava.py): Llama decoder and sampler --------------------------------------------------
+ * uav_rmsnorm: transformers LlamaRMSNorm on fp16 [rows][ld] rows of C % 8 == 0 columns: fp32 mean of squares,
+ *   x * rsqrt(var + eps) rounded to fp16, then times the fp16 weight in fp16 */
+uav_status_t uav_rmsnorm(const void* x, int64_t rows, int64_t C, int64_t ldx, const void* weight, float eps, void* out,
+                         int64_t ldo, uav_stream_t stream);
+/* rotate-half rotary embedding of head_dim 128 on the q and k columns of n fused q|k|v fp16 rows ([n][ld_qkv]: q at
+ * columns [0, C), k at [C, 2C), v at [2C, 3C), C = heads * 128) at positions [p0, p0 + n): q is rotated in place, the
+ * rotated k and v go to rows [p0, p0 + n) of k_cache / v_cache ([cache_rows][ld_kv] fp16).  cos_sin: fp32
+ * [positions][64][2] = cos, sin of position * inv_freq[i] */
+uav_status_t uav_rope_kv_append(void* qkv, int64_t ld_qkv, int64_t n, int heads, int head_dim, int64_t p0,
+                                const float* cos_sin, int64_t positions, void* k_cache, void* v_cache, int64_t ld_kv,
+                                int64_t cache_rows, uav_stream_t stream);
+/* out[r][c] = silu(gate_up[r][c]) * gate_up[r][inter + c] (transformers LlamaMLP on the fused gate|up output), fp16 */
+uav_status_t uav_swiglu(const void* gate_up, int64_t ld_gu, int64_t rows, int64_t inter, void* out, int64_t ldo,
+                        uav_stream_t stream);
+/* one-row GEMV, the decode step's weight stream: out[n] = sum_k w[n][k] x[k] (+ residual[n]), w fp16 [N][K] dense,
+ * x fp16 [K], fp32 accumulation; out_dtype UAV_F16 (residual fp16 or NULL) or UAV_F32 (no residual).  K % 8 == 0,
+ * K <= 16384.  Split-K over the warps of a row with a fixed-order combine: deterministic. */
+uav_status_t uav_gemv(const void* w, int64_t N, int64_t K, const void* x, const void* residual, void* out, int out_dtype,
+                      uav_stream_t stream);
+/* attention of one query row per head (q fp16 [heads * 128]) against the first L rows of a KV cache ([L][ld_kv] fp16),
+ * out fp16 [heads * 128]; key chunks are combined in a fixed order (flash-decoding).  workspace: fp32 scratch of
+ * uav_attention_decode_workspace_bytes(heads, L) bytes */
+size_t uav_attention_decode_workspace_bytes(int heads, int64_t L);
+uav_status_t uav_attention_decode(const void* q, const void* k_cache, const void* v_cache, int64_t ld_kv, int64_t L,
+                                  int heads, int head_dim, float scale, void* out, void* workspace, size_t ws_bytes,
+                                  uav_stream_t stream);
+/* next token from fp32 logits [V] (V <= 49152): temperature, then transformers TopPLogitsWarper's keep rule, then the
+ * inverse CDF of the kept set in vocabulary order at u * (kept mass), u in [0, 1).  temperature == 0: argmax, first
+ * index on ties.  The token id is written to *token (device int64). */
+uav_status_t uav_sample_top_p(const float* logits, int64_t V, float temperature, float top_p, float u, int64_t* token,
+                              uav_stream_t stream);
 
 #ifdef __cplusplus
 }

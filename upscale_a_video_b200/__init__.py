@@ -2,7 +2,7 @@
 
 Public surface mirrors the reference (`/root/reference/models_video/`): `VideoUpscalePipeline`,
 `UNetVideoModel`, `AutoencoderKLVideo`, `DDIMScheduler`, `Propagation`, `RAFT_bi` (models_video/RAFT/raft_bi.py) and the
-`CLIPTextModel` the pipeline holds as `text_encoder`.  The arithmetic runs in
+`CLIPTextModel` the pipeline holds as `text_encoder`, plus `LLavaAgent` (llava/llava_agent.py), the LLaVA-1.5 captioner.  The arithmetic runs in
 hand-written CUDA kernels behind a C ABI (`include/uav_b200.h`, `csrc/`); there is no CPU path.
 """
 __version__ = "0.1.0"
@@ -19,6 +19,7 @@ _LAZY = {
     "initialize_RAFT": "raft",
     "CLIPTextModel": "clip_text",
     "CLIPTextConfig": "clip_text",
+    "LLavaAgent": "llava",
 }
 
 

@@ -105,6 +105,12 @@ _PROTOS = {
     "uav_pack_video_uint8": [P, I64, I64, I64, I64, P, P],
     "uav_pack_frames_png": [P, I64, I64, I64, I64, P, P],
     "uav_unpack_video_uint8": [P, I64, I64, I64, I64, I64, I32, P, P],
+    "uav_rmsnorm": [P, I64, I64, I64, P, F32, P, I64, P],
+    "uav_rope_kv_append": [P, I64, I64, I32, I32, I64, P, I64, P, P, I64, I64, P],
+    "uav_swiglu": [P, I64, I64, I64, P, I64, P],
+    "uav_gemv": [P, I64, I64, P, P, P, I32, P],
+    "uav_attention_decode": [P, P, P, I64, I64, I32, I32, F32, P, P, C.c_size_t, P],
+    "uav_sample_top_p": [P, I64, F32, F32, F32, P, P],
 }
 _SPECIAL = {
     "uav_version": (C.c_char_p, []),
@@ -114,6 +120,7 @@ _SPECIAL = {
     "uav_gn_partial_blocks": (C.c_int64, [I64, I64, I64]),
     "uav_plane_stats_workspace_bytes": (C.c_size_t, [I64]),
     "uav_instnorm_workspace_bytes": (C.c_size_t, [I64, I64]),
+    "uav_attention_decode_workspace_bytes": (C.c_size_t, [I32, I64]),
 }
 
 

@@ -12,14 +12,20 @@ writes.  No buffer at output resolution holds more than one 3-frame chunk, so me
 beyond the low-resolution sampling state.  Under `torchrun` (WORLD_SIZE > 1) each process drives the GPU LOCAL_RANK
 and the pipeline's tile / window sharding splits the work; only rank 0 writes files.
 
-Deliberate differences from the reference CLI (INTEGRATION.md §3): there is no LLaVA captioner (`--caption` supplies
-the caption text), errors raise instead of being printed, `--save_image` writes one PNG per frame, the mp4 codec is
+With `--llava_path` (and without `--no_llava`) frame 0 of each clip is captioned by `llava.LLavaAgent` before the
+upscale, with the reference's preprocessing and a generator seeded from SEED; the prompt is `caption + a_prompt`.  Under
+`torchrun` only rank 0 loads and runs the captioner and the caption is broadcast to the other ranks.
+
+Deliberate differences from the reference CLI (INTEGRATION.md §3): the captioner runs only when `--llava_path` names a
+LLaVA-1.5 folder (otherwise `--caption` supplies the caption text), its sampling is seeded, errors raise instead of
+being printed, `--save_image` writes one PNG per frame, the mp4 codec is
 mp4v, and the tiling decision is taken per clip."""
 from __future__ import annotations
 
 import argparse
 import contextlib
 import os
+import textwrap
 import time
 from typing import Iterator, List, Optional, Tuple
 
@@ -53,8 +59,13 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--n_prompt", type=str, default="blur, worst quality")
     p.add_argument("--use_video_vae", action="store_true", default=False)
     p.add_argument("--color_fix", type=str, default="None", choices=["None", "AdaIn", "Wavelet"])
-    p.add_argument("--no_llava", action="store_true", default=False, help="Accepted for compatibility; there is no captioner.")
-    p.add_argument("--load_8bit_llava", action="store_true", default=False, help="Not supported: there is no captioner.")
+    p.add_argument("--no_llava", action="store_true", default=False, help="Do not caption, even with --llava_path.")
+    p.add_argument("--load_8bit_llava", action="store_true", default=False,
+                   help="Not supported: the captioner runs in fp16.")
+    p.add_argument("--llava_path", type=str, default=None,
+                   help="LLaVA-1.5 folder (released format): caption frame 0 of each clip with it.")
+    p.add_argument("--llava_vision_path", type=str, default=None,
+                   help="CLIP ViT-L/14-336 folder of the captioner's vision tower (default: the config's mm_vision_tower).")
     p.add_argument("--perform_tile", action="store_true", default=False)
     p.add_argument("--tile_size", type=int, default=256)
     p.add_argument("--save_image", action="store_true", default=False)
@@ -70,8 +81,33 @@ def parse_args(argv: Optional[List[str]] = None) -> argparse.Namespace:
     parser = build_parser()
     args = parser.parse_args(argv)
     if args.load_8bit_llava:
-        parser.error("--load_8bit_llava: there is no LLaVA captioner in this package; pass the caption with --caption")
+        parser.error("--load_8bit_llava: there is no LLaVA captioner for 8-bit weights; it runs in fp16")
+    if args.caption and use_llava(args):
+        parser.error("--caption and --llava_path both give the caption: pass one of them (or --no_llava)")
     return args
+
+
+def use_llava(args: argparse.Namespace) -> bool:
+    return args.llava_path is not None and not args.no_llava
+
+
+def caption_frame(agent, frame_bgr: np.ndarray) -> str:
+    """inference_upscale_a_video.py:158-175: the caption of a clip's first frame, sampled from a generator seeded with
+    SEED so that a rerun gives the same caption"""
+    from .llava import frame0_image
+    img = frame0_image(np.ascontiguousarray(frame_bgr[..., ::-1]))
+    return agent.gen_image_caption([img], generator=torch.Generator().manual_seed(SEED))[0]
+
+
+def _shared_caption(agent, frame_bgr, rank: int) -> str:
+    """rank 0 captions; under torch.distributed every rank gets its caption"""
+    import torch.distributed as dist
+    caption = caption_frame(agent, frame_bgr) if rank == 0 else None
+    if dist.is_initialized() and dist.get_world_size() > 1:
+        box = [caption]
+        dist.broadcast_object_list(box, src=0)
+        caption = box[0]
+    return caption
 
 
 def save_name(video_name: str, args: argparse.Namespace) -> str:
@@ -189,11 +225,21 @@ def main(argv: Optional[List[str]] = None) -> List[str]:
         log = print if rank == 0 else (lambda *a, **k: None)
         log("Loading Upscale-A-Video")
         pipeline, raft = load_models(args, paths, device)
+        agent = None
+        if use_llava(args) and rank == 0:
+            from .llava import LLavaAgent
+            log("Loading LLaVA")
+            agent = LLavaAgent(args.llava_path, device=device, vision_tower_path=args.llava_vision_path)
         written = []
         for i, video_path in enumerate(video_list):
             frames, fps, video_name = video_io.read_frames(video_path)
             index_str = f"[{i + 1}/{len(video_list)}]"
             log(f"{index_str} Processing video: ", video_name)
+            caption = args.caption
+            if use_llava(args):
+                log(f"{index_str} Generating video caption with LLaVA...")
+                caption = _shared_caption(agent, frames[0], rank)
+                log(textwrap.indent(textwrap.fill("Caption: " + caption, width=80), " " * 8))
             vframes = ingest_frames(frames, device, from_video=video_io.is_video(video_path))
             video_path_out, frame_dir = output_paths(args, video_name)
             writer = None
@@ -204,7 +250,7 @@ def main(argv: Optional[List[str]] = None) -> List[str]:
             start, write_time = time.time(), 0.0
             try:
                 with writer or contextlib.nullcontext():
-                    for s, _, output in upscale_clip(pipeline, raft, vframes, args, args.caption + args.a_prompt,
+                    for s, _, output in upscale_clip(pipeline, raft, vframes, args, caption + args.a_prompt,
                                                      fix_colors=rank == 0):
                         if writer is None:
                             continue

@@ -17,7 +17,21 @@ from torch import nn
 from . import _lib, ops
 from .layers import PackedModule
 
-__all__ = ["CLIPTextConfig", "CLIPTextModel"]
+__all__ = ["CLIPTextConfig", "CLIPTextModel", "encoder_layer"]
+
+
+def encoder_layer(x: torch.Tensor, w, heads: int, eps: float, act: int, causal: bool) -> torch.Tensor:
+    """one pre-LayerNorm CLIP encoder layer on x (b, n, hidden) fp16, shared by the text encoder (causal) and LLaVA's
+    vision tower (llava.py, bidirectional).  `w` holds the kernel-ready weights: ln1 / ln2 (fp32 gamma, beta), qkv, out,
+    fc1, fc2 (fp16 weight, fp32 bias or None), the q|k|v projections row-concatenated."""
+    hidden = x.shape[-1]
+    h = ops.layer_norm(x, *w.ln1, eps)
+    qkv = ops.linear(h, *w.qkv)
+    attn = ops.attention_causal if causal else ops.attention
+    o = attn(qkv[..., :hidden], qkv[..., hidden:2 * hidden], qkv[..., 2 * hidden:], heads)
+    x = ops.linear(o, *w.out, residual=x)
+    h = ops.layer_norm(x, *w.ln2, eps)
+    return ops.linear(ops.linear(h, *w.fc1, act=act), *w.fc2, residual=x)
 
 
 class CLIPTextConfig(SimpleNamespace):
@@ -131,22 +145,14 @@ class CLIPTextModel(PackedModule):
         pos = pk.tensor("pos16", lambda: tm.embeddings.position_embedding.weight.detach().to(torch.float16))
         # embeddings: fp32 sum of the two fp16 table rows, one rounding
         x = (tok.index_select(0, input_ids.reshape(-1).to(dev)).float().view(b, n, -1) + pos[:n].float()[None]).to(torch.float16)
-        hidden, heads = cfg.hidden_size, cfg.num_attention_heads
+        heads = cfg.num_attention_heads
         act = ops.ACT_GELU if cfg.hidden_act == "gelu" else ops.ACT_QUICK_GELU
         for i, layer in enumerate(tm.encoder.layers):
             a = layer.self_attn
-            g1, b1 = pk.affine(layer.layer_norm1)
-            h = ops.layer_norm(x, g1, b1, cfg.layer_norm_eps)
-            wqkv, bqkv = pk.fused_linear(f"qkv{i}", [a.q_proj, a.k_proj, a.v_proj])
-            qkv = ops.linear(h, wqkv, bqkv)
-            o = ops.attention_causal(qkv[..., :hidden], qkv[..., hidden:2 * hidden], qkv[..., 2 * hidden:], heads)
-            wo, bo = pk.linear(a.out_proj)
-            x = ops.linear(o, wo, bo, residual=x)
-            g2, b2 = pk.affine(layer.layer_norm2)
-            h = ops.layer_norm(x, g2, b2, cfg.layer_norm_eps)
-            w1, bb1 = pk.linear(layer.mlp.fc1)
-            w2, bb2 = pk.linear(layer.mlp.fc2)
-            x = ops.linear(ops.linear(h, w1, bb1, act=act), w2, bb2, residual=x)
+            w = SimpleNamespace(ln1=pk.affine(layer.layer_norm1), qkv=pk.fused_linear(f"qkv{i}", [a.q_proj, a.k_proj, a.v_proj]),
+                                out=pk.linear(a.out_proj), ln2=pk.affine(layer.layer_norm2), fc1=pk.linear(layer.mlp.fc1),
+                                fc2=pk.linear(layer.mlp.fc2))
+            x = encoder_layer(x, w, heads, cfg.layer_norm_eps, act, causal=True)
         gf, bf = pk.affine(tm.final_layer_norm)
         out = ops.layer_norm(x, gf, bf, cfg.layer_norm_eps)
         return out.to(self.dtype), None

@@ -543,7 +543,7 @@ __global__ void __launch_bounds__(128)
 uav_status_t attention_tc(const void* q, const void* k, const void* v, void* out, int64_t batch,
                           int heads, int head_dim, int64_t nq, int64_t nk, int64_t ldq, int64_t ldk,
                           int64_t ldv, int64_t ldo, int64_t kv_batch_div, float scale,
-                          cudaStream_t stream);  // attention_tc.cu (wgmma)
+                          cudaStream_t stream, bool causal = false);  // attention_tc.cu (wgmma)
 
 template <int D, int NB16>
 static uav_status_t launch_cross(const FaParams& p, int batch, cudaStream_t stream) {

@@ -4,7 +4,9 @@
 //     320x576 -> 70 TFLOP per frame, 71 % of VAE-decode FLOPs): fa_tc_kernel<512, 256, 64>;
 //   * UNet spatial self-attention: 8 heads, d = 128, N = 2880: fa_tc_kernel<128, 128, 128>.
 // d = 64 (no pipeline shape: the UNet's d = 64 attention is text cross-attention, attention.cu) runs on
-// fa_tc_kernel<64, 64, 128>.
+// fa_tc_kernel<64, 64, 128>.  Causal self-attention with d = 128 over more than 128 tokens (the LLaVA decoder's prefill,
+// llava.py) runs on fa_tc_causal_kernel<128, 128, 128>: the same body, which skips the key tiles past the diagonal and
+// masks the keys after each query row in the diagonal tile.
 //
 // One CTA = 128 query rows x DVT output columns; warpgroup 0 is the TMA producer (one thread), warpgroups 1 and 2 each
 // own 64 query rows.  Per kv tile of BN rows a consumer warpgroup computes S = Q K^T with wgmma from shared memory
@@ -48,9 +50,8 @@ struct FaTcCfg {
   static constexpr int SMEM_BYTES = Q_BYTES + STAGES * SLOT_BYTES + 1024 + 1024;
 };
 
-template <int DQK, int DVT, int BN>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-    fa_tc_kernel(const __grid_constant__ FaTcParams p) {
+template <int DQK, int DVT, int BN, bool CAUSAL>
+__device__ __forceinline__ void fa_tc_body(const FaTcParams& p) {
   using Cfg = FaTcCfg<DQK, DVT, BN>;
   constexpr int STAGES = Cfg::STAGES;
   constexpr int QSLABS = Cfg::QSLABS;
@@ -68,7 +69,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
   const int bh = blockIdx.z;
   const int b = bh / p.heads, h = bh % p.heads;
   const int bkv = b / p.kv_batch_div;
-  const int ntiles = (p.nk + BN - 1) / BN;
+  int ntiles = (p.nk + BN - 1) / BN;
+  if constexpr (CAUSAL) ntiles = min(ntiles, (q0 + TC_BM + BN - 1) / BN);  // no key of a later tile is <= a row of this CTA
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.map_q);
@@ -141,6 +143,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i)
         if (8 * (i / 4) + 2 * lr + (i % 2) >= valid) s[i] = -INFINITY;
+    }
+    if constexpr (CAUSAL) {
+      // key j * BN + col is masked for query row q0 + row0 + 8 ((i / 2) % 2) when it lies after the row; key 0 is in the
+      // first tile, so every row keeps a finite maximum
+      const int row0 = q0 + 64 * wg + 16 * (warp_idx & 3) + lq - j * BN;
+      if (j * BN + BN - 1 > q0 + 64 * wg) {
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i)
+          if (8 * (i / 4) + 2 * lr + (i % 2) > row0 + 8 * ((i / 2) & 1)) s[i] = -INFINITY;
+      }
     }
     float alpha[2], neg_m[2];
 #pragma unroll
@@ -215,20 +227,36 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
   }
 }
 
+template <int DQK, int DVT, int BN>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+    fa_tc_kernel(const __grid_constant__ FaTcParams p) {
+  fa_tc_body<DQK, DVT, BN, false>(p);
+}
 
 template <int DQK, int DVT, int BN>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+    fa_tc_causal_kernel(const __grid_constant__ FaTcParams p) {
+  fa_tc_body<DQK, DVT, BN, true>(p);
+}
+
+
+template <int DQK, int DVT, int BN, bool CAUSAL = false>
 static uav_status_t launch_fa_tc(FaTcParams& p, int64_t batch, int dv_splits, cudaStream_t stream) {
   const dim3 grid((p.nq + TC_BM - 1) / TC_BM, dv_splits, (unsigned)(batch * p.heads));
-  return launch_opted_in<fa_tc_kernel<DQK, DVT, BN>>(grid, TC_THREADS, FaTcCfg<DQK, DVT, BN>::SMEM_BYTES, stream, p);
+  if constexpr (CAUSAL)
+    return launch_opted_in<fa_tc_causal_kernel<DQK, DVT, BN>>(grid, TC_THREADS, FaTcCfg<DQK, DVT, BN>::SMEM_BYTES,
+                                                              stream, p);
+  else
+    return launch_opted_in<fa_tc_kernel<DQK, DVT, BN>>(grid, TC_THREADS, FaTcCfg<DQK, DVT, BN>::SMEM_BYTES, stream, p);
 }
 
 
 // entry used by uav_attention (attention.cu), which has validated the arguments, for head_dim 64, 128 and 512 (one
-// head)
+// head), and by uav_attention_causal (clip_text.cu) for head_dim 128 with causal = true and nq = nk
 uav_status_t attention_tc(const void* q, const void* k, const void* v, void* out, int64_t batch,
                           int heads, int head_dim, int64_t nq, int64_t nk, int64_t ldq, int64_t ldk,
                           int64_t ldv, int64_t ldo, int64_t kv_batch_div, float scale,
-                          cudaStream_t stream) {
+                          cudaStream_t stream, bool causal) {
   FaTcParams p;
   memset(&p, 0, sizeof(p));
   const int64_t C = (int64_t)heads * head_dim;
@@ -254,6 +282,7 @@ uav_status_t attention_tc(const void* q, const void* k, const void* v, void* out
   p.heads = heads;
   p.kv_batch_div = (int)kv_batch_div;
   p.scale_log2 = scale * 1.4426950408889634f;
+  if (causal) return launch_fa_tc<128, 128, 128, true>(p, batch, 1, stream);
   if (head_dim == 512) return launch_fa_tc<512, 256, 64>(p, batch, 2, stream);
   if (head_dim == 64) return launch_fa_tc<64, 64, 128>(p, batch, 1, stream);
   return launch_fa_tc<128, 128, 128>(p, batch, 1, stream);

@@ -4,8 +4,8 @@
 #include "uav_common.cuh"
 
 // ---------------------------------------------------------------------------------------
-// CLIP text encoder (SURVEY.md §8f rank 3): causal self-attention over a short sequence (77 tokens) — the only attention
-// on the path that needs a mask.  One CTA per (batch, head): K and V of the head in shared memory, one warp per query row,
+// CLIP text encoder (SURVEY.md §8f rank 3): causal self-attention over a short sequence (77 tokens).  Longer sequences
+// with head_dim 128 (the LLaVA decoder's prefill) run on the causal wgmma kernel of attention_tc.cu.  One CTA per (batch, head): K and V of the head in shared memory, one warp per query row,
 // lane j scores key j (j <= i), fp32 softmax, then lanes own output columns.  n <= 128, d <= 128, d % 2 == 0.
 // (transformers CLIPAttention with the causal mask of CLIPTextTransformer; run once per prompt: clarity over speed.)
 // ---------------------------------------------------------------------------------------
@@ -76,6 +76,10 @@ __global__ void __launch_bounds__(128)
     __syncwarp();
   }
 }
+uav_status_t attention_tc(const void* q, const void* k, const void* v, void* out, int64_t batch,
+                          int heads, int head_dim, int64_t nq, int64_t nk, int64_t ldq, int64_t ldk,
+                          int64_t ldv, int64_t ldo, int64_t kv_batch_div, float scale,
+                          cudaStream_t stream, bool causal);  // attention_tc.cu (wgmma)
 }  // namespace uav
 
 extern "C" {
@@ -84,8 +88,22 @@ uav_status_t uav_attention_causal(const void* q, const void* k, const void* v, v
                                   int64_t n, int64_t ldq, int64_t ldk, int64_t ldv, int64_t ldo, float scale,
                                   uav_stream_t stream) {
   UAV_REQUIRE(q && k && v && out && batch > 0 && heads > 0, "uav_attention_causal: bad argument");
+  if (head_dim == 128 && n > uav::CA_MAX_N) {
+    UAV_REQUIRE(n <= INT32_MAX && batch * heads <= 65535, "uav_attention_causal: n or batch*heads too large");
+    UAV_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0,
+                "uav_attention_causal: token strides must be multiples of 8");
+    UAV_REQUIRE(scale > 0.f && scale < INFINITY, "uav_attention_causal: scale must be finite and > 0 (got %g)",
+                (double)scale);
+    UAV_REQUIRE_ALIGNED16("uav_attention_causal", q);
+    UAV_REQUIRE_ALIGNED16("uav_attention_causal", k);
+    UAV_REQUIRE_ALIGNED16("uav_attention_causal", v);
+    UAV_REQUIRE_ALIGNED16("uav_attention_causal", out);
+    return uav::attention_tc(q, k, v, out, batch, heads, head_dim, n, n, ldq, ldk, ldv, ldo, 1, scale,
+                             (cudaStream_t)stream, true);
+  }
   UAV_REQUIRE(n >= 1 && n <= uav::CA_MAX_N && head_dim >= 2 && head_dim <= 128 && head_dim % 2 == 0,
-              "uav_attention_causal: sequence <= %d tokens and even head_dim <= 128 (got n=%lld d=%d)", uav::CA_MAX_N,
+              "uav_attention_causal: sequence <= %d tokens (any length for head_dim 128) and even head_dim <= 128 "
+              "(got n=%lld d=%d)", uav::CA_MAX_N,
               (long long)n, head_dim);
   UAV_REQUIRE(batch <= 65535, "uav_attention_causal: batch too large");
   const uav_status_t st = uav::opt_in_smem<uav::causal_attn_kernel>((int)uav::ca_smem_bytes(uav::CA_MAX_N, 128));

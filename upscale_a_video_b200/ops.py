@@ -909,3 +909,93 @@ def attention_causal(q, k, v, heads: int, *, scale: Optional[float] = None, out=
                                         q.stride(1), k.stride(1), v.stride(1), out.stride(1), scale, _stream()),
                "uav_attention_causal")
     return out
+
+
+# ---------------------------------------------------------------------------------------
+# LLaVA-1.5 captioner (llava.py): the Llama decoder's kernels and the sampler
+# ---------------------------------------------------------------------------------------
+def _rows(x: torch.Tensor):
+    """(rows, row stride) of a 2-D fp16 tensor whose last dim is dense"""
+    assert x.is_cuda and x.dtype == torch.float16 and x.dim() == 2 and x.stride(-1) == 1
+    return x.shape[0], x.stride(0)
+
+
+def rms_norm(x: torch.Tensor, weight: torch.Tensor, eps: float, out=None):
+    """transformers LlamaRMSNorm of the rows of x (rows, C) fp16 (a row slice or column slice allowed); weight fp16 (C,)"""
+    rows, ldx = _rows(x)
+    assert weight.dtype == torch.float16 and weight.is_contiguous() and weight.numel() == x.shape[1]
+    if out is None:
+        out = torch.empty(x.shape, dtype=torch.float16, device=x.device)
+    _, ldo = _rows(out)
+    with _timed("rmsnorm", 0.0, 2.0 * 2 * x.numel()):
+        _lib.check(_lib.load().uav_rmsnorm(x.data_ptr(), rows, x.shape[1], ldx, weight.data_ptr(), eps, out.data_ptr(),
+                                           ldo, _stream()), "uav_rmsnorm")
+    return out
+
+
+def rope_kv_append(qkv: torch.Tensor, heads: int, p0: int, cos_sin: torch.Tensor, k_cache: torch.Tensor,
+                   v_cache: torch.Tensor):
+    """rotate q (in place) and k of the fused q|k|v rows qkv (n, >= 3 heads 128) at positions [p0, p0 + n); rotated k
+    and v go to rows [p0, p0 + n) of k_cache / v_cache (L_max, heads 128).  cos_sin: fp32 (positions, 64, 2)"""
+    n, ld = _rows(qkv)
+    rows, ld_kv = _rows(k_cache)
+    assert v_cache.shape == k_cache.shape and v_cache.stride() == k_cache.stride()
+    assert cos_sin.dtype == torch.float32 and cos_sin.is_contiguous() and cos_sin.shape[1:] == (64, 2)
+    _lib.check(_lib.load().uav_rope_kv_append(qkv.data_ptr(), ld, n, heads, 128, p0, cos_sin.data_ptr(), cos_sin.shape[0],
+                                              k_cache.data_ptr(), v_cache.data_ptr(), ld_kv, rows, _stream()),
+               "uav_rope_kv_append")
+
+
+def swiglu(gate_up: torch.Tensor, out=None):
+    """silu(gate) * up of the fused (rows, 2 I) gate|up GEMM output -> (rows, I) fp16"""
+    rows, ld = _rows(gate_up)
+    inter = gate_up.shape[1] // 2
+    if out is None:
+        out = torch.empty(rows, inter, dtype=torch.float16, device=gate_up.device)
+    _, ldo = _rows(out)
+    _lib.check(_lib.load().uav_swiglu(gate_up.data_ptr(), ld, rows, inter, out.data_ptr(), ldo, _stream()), "uav_swiglu")
+    return out
+
+
+def gemv(w: torch.Tensor, x: torch.Tensor, *, residual=None, out=None, out_dtype=torch.float16):
+    """out (N,) = w (N, K) @ x (K,) (+ residual (N,)), the one-row weight stream of a decode step; fp16 or fp32 out"""
+    assert w.is_cuda and w.dtype == torch.float16 and w.is_contiguous() and w.dim() == 2
+    N, K = w.shape
+    assert x.dtype == torch.float16 and x.numel() == K and x.is_contiguous()
+    if out is None:
+        out = torch.empty(N, dtype=out_dtype, device=w.device)
+    assert out.numel() == N and out.is_contiguous() and out.dtype in (torch.float16, torch.float32)
+    if residual is not None:
+        assert residual.dtype == torch.float16 and residual.numel() == N and residual.is_contiguous()
+    with _timed("gemv", 2.0 * N * K, 2.0 * (N * K + K + N), f"gemv N{N} K{K}"):
+        _lib.check(_lib.load().uav_gemv(w.data_ptr(), N, K, x.data_ptr(), 0 if residual is None else residual.data_ptr(),
+                                        out.data_ptr(), F16 if out.dtype == torch.float16 else F32, _stream()),
+                   "uav_gemv")
+    return out
+
+
+def attention_decode(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, L: int, heads: int, *,
+                     scale: Optional[float] = None, out=None):
+    """one query row q (heads 128,) fp16 against rows [0, L) of the KV cache (L_max, heads 128) -> (heads 128,) fp16"""
+    _, ld_kv = _rows(k_cache)
+    assert v_cache.stride() == k_cache.stride() and q.dtype == torch.float16 and q.is_contiguous()
+    if out is None:
+        out = torch.empty(heads * 128, dtype=torch.float16, device=q.device)
+    lib = _lib.load()
+    ws_bytes = int(lib.uav_attention_decode_workspace_bytes(heads, L))
+    ws = torch.empty(ws_bytes // 4, dtype=torch.float32, device=q.device)
+    _lib.check(lib.uav_attention_decode(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), ld_kv, L, heads, 128,
+                                        128 ** -0.5 if scale is None else scale, out.data_ptr(), ws.data_ptr(), ws_bytes,
+                                        _stream()), "uav_attention_decode")
+    return out
+
+
+def sample_top_p(logits: torch.Tensor, temperature: float, top_p: float, u: float, out=None) -> torch.Tensor:
+    """next token id (a device int64 scalar) from fp32 logits (V,): temperature, top-p nucleus, inverse CDF at u in
+    [0, 1); temperature 0 = argmax (first index on ties)"""
+    assert logits.is_cuda and logits.dtype == torch.float32 and logits.is_contiguous()
+    if out is None:
+        out = torch.empty((), dtype=torch.int64, device=logits.device)
+    _lib.check(_lib.load().uav_sample_top_p(logits.data_ptr(), logits.numel(), temperature, top_p, u, out.data_ptr(),
+                                            _stream()), "uav_sample_top_p")
+    return out
