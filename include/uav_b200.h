@@ -430,6 +430,15 @@ uav_status_t uav_rmsnorm(const void* x, int64_t rows, int64_t C, int64_t ldx, co
 uav_status_t uav_rope_kv_append(void* qkv, int64_t ld_qkv, int64_t n, int heads, int head_dim, int64_t p0,
                                 const float* cos_sin, int64_t positions, void* k_cache, void* v_cache, int64_t ld_kv,
                                 int64_t cache_rows, uav_stream_t stream);
+/* uav_rope_kv_append on `batch` sequences at once (n rows each, positions [p0, p0 + n) in every sequence): sequence b's
+ * rows start at qkv + b * qkv_batch_stride and its caches at k_cache / v_cache + b * kv_batch_stride (elements), each
+ * [cache_rows][ld_kv].  Serves the prefill (n = prompt length) and every decode step (n = 1); each sequence's result
+ * is bit-identical to a uav_rope_kv_append call on it alone.  batch > 1 needs qkv_batch_stride >= n * ld_qkv and
+ * kv_batch_stride >= cache_rows * ld_kv. */
+uav_status_t uav_rope_kv_append_batched(void* qkv, int64_t ld_qkv, int64_t qkv_batch_stride, int64_t batch, int64_t n,
+                                        int heads, int head_dim, int64_t p0, const float* cos_sin, int64_t positions,
+                                        void* k_cache, void* v_cache, int64_t ld_kv, int64_t kv_batch_stride,
+                                        int64_t cache_rows, uav_stream_t stream);
 /* out[r][c] = silu(gate_up[r][c]) * gate_up[r][inter + c] (transformers LlamaMLP on the fused gate|up output), fp16 */
 uav_status_t uav_swiglu(const void* gate_up, int64_t ld_gu, int64_t rows, int64_t inter, void* out, int64_t ldo,
                         uav_stream_t stream);
@@ -438,6 +447,11 @@ uav_status_t uav_swiglu(const void* gate_up, int64_t ld_gu, int64_t rows, int64_
  * K <= 16384.  Split-K over the warps of a row with a fixed-order combine: deterministic. */
 uav_status_t uav_gemv(const void* w, int64_t N, int64_t K, const void* x, const void* residual, void* out, int out_dtype,
                       uav_stream_t stream);
+/* uav_gemv on 1 <= rows <= 8 input rows with w streamed once for all of them: out[r][n] = sum_k w[n][k] x[r][k]
+ * (+ residual[r][n]); x fp16 [rows][K], residual fp16 [rows][N] and out [rows][N] dense.  rows * K <= 110592 when
+ * rows > 1 (x is held in shared memory).  Each row's result is bit-identical to uav_gemv on that row. */
+uav_status_t uav_gemv_rows(const void* w, int64_t N, int64_t K, const void* x, int64_t rows, const void* residual,
+                           void* out, int out_dtype, uav_stream_t stream);
 /* attention of one query row per head (q fp16 [heads * 128]) against the first L rows of a KV cache ([L][ld_kv] fp16),
  * out fp16 [heads * 128]; key chunks are combined in a fixed order (flash-decoding).  workspace: fp32 scratch of
  * uav_attention_decode_workspace_bytes(heads, L) bytes */
@@ -445,11 +459,26 @@ size_t uav_attention_decode_workspace_bytes(int heads, int64_t L);
 uav_status_t uav_attention_decode(const void* q, const void* k_cache, const void* v_cache, int64_t ld_kv, int64_t L,
                                   int heads, int head_dim, float scale, void* out, void* workspace, size_t ws_bytes,
                                   uav_stream_t stream);
+/* uav_attention_decode for `batch` sequences that share the cache length L: sequence b's query row is q + b * ldq,
+ * its caches k_cache / v_cache + b * kv_batch_stride (elements) and its output out + b * ldo.  Each sequence's result
+ * is bit-identical to uav_attention_decode on it alone.  batch > 1 needs ldq, ldo >= heads * 128, ldq % 4 == 0 and
+ * kv_batch_stride >= L * ld_kv, % 4 == 0.  workspace: uav_attention_decode_batched_workspace_bytes(batch, heads, L) */
+size_t uav_attention_decode_batched_workspace_bytes(int64_t batch, int heads, int64_t L);
+uav_status_t uav_attention_decode_batched(const void* q, int64_t ldq, const void* k_cache, const void* v_cache,
+                                          int64_t ld_kv, int64_t kv_batch_stride, int64_t batch, int64_t L, int heads,
+                                          int head_dim, float scale, void* out, int64_t ldo, void* workspace,
+                                          size_t ws_bytes, uav_stream_t stream);
 /* next token from fp32 logits [V] (V <= 49152): temperature, then transformers TopPLogitsWarper's keep rule, then the
  * inverse CDF of the kept set in vocabulary order at u * (kept mass), u in [0, 1).  temperature == 0: argmax, first
  * index on ties.  The token id is written to *token (device int64). */
 uav_status_t uav_sample_top_p(const float* logits, int64_t V, float temperature, float top_p, float u, int64_t* token,
                               uav_stream_t stream);
+/* uav_sample_top_p on 1 <= rows <= 8 rows of fp32 logits ([rows][ld_logits]), one CTA per row: row r is sampled
+ * with the host uniform u[r] (read before the call returns: no device copy) into tokens[r].  Each row's token is the
+ * one uav_sample_top_p picks for that row. */
+uav_status_t uav_sample_top_p_batched(const float* logits, int64_t ld_logits, int64_t rows, int64_t V,
+                                      float temperature, float top_p, const float* u, int64_t* tokens,
+                                      uav_stream_t stream);
 
 #ifdef __cplusplus
 }

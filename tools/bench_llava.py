@@ -4,7 +4,11 @@ tokens, and `uav_gemv` GB/s per decode shape against the H100 SXM data sheet's 3
 importable, `LlamaForCausalLM.generate` (fp16, greedy, 64 new tokens) on the same weights is timed in the same run as a
 baseline.  Prints the card's name and power limit first.
 
-    python tools/bench_llava.py [--layers 40] [--json out.json]
+With `--rows 1,2,4,8`, for each row count B: `uav_gemv_rows` µs and GB/s at the five decode shapes, ms per batched
+decode step (B rows, one weight pass), and seconds for one `generate_ids_batch` call captioning B images (vision tower,
+prefill, 64 sampled tokens per row).
+
+    python tools/bench_llava.py [--layers 40] [--rows 1,2,4,8] [--json out.json]
 """
 import argparse
 import json
@@ -85,15 +89,90 @@ def bench_gemv():
     return rows
 
 
+def bench_gemv_rows(rows):
+    from upscale_a_video_b200 import ops
+    out_rows = []
+    for N, K in ((3 * H, H), (H, H), (2 * INTER, H), (H, INTER), (VOCAB, H)):
+        w = torch.randn(N, K, device="cuda", dtype=torch.float16)
+        x = torch.randn(rows, K, device="cuda", dtype=torch.float16)
+        out = torch.empty(rows, N, device="cuda", dtype=torch.float16)
+        for _ in range(5):
+            ops.gemv_rows(w, x, out=out)
+        ms = events_ms(lambda: ops.gemv_rows(w, x, out=out), 200)
+        gbs = N * K * 2 / (ms * 1e-3) / 1e9
+        out_rows.append(dict(N=N, K=K, us=ms * 1e3, GBs=gbs, of_peak=gbs / (HBM_TBS * 1e3)))
+        del w
+    return out_rows
+
+
+def bench_rows(agent, px, ids, rows):
+    """decode ms per step of `rows` sequences and seconds of one caption call on `rows` images"""
+    pxb = px[None].expand(rows, -1, -1, -1).contiguous()
+    with torch.no_grad():
+        x = agent.embed_prompt(ids, agent.vision_features(pxb))
+        tok = torch.full((rows,), 29871, dtype=torch.int64, device="cuda")
+
+        def run(max_new):
+            for _ in agent._run(x, max_new, lambda step, logits: tok):
+                pass
+
+        run(2)
+        prefill = events_ms(lambda: run(1), 2)
+        step_ms = (events_ms(lambda: run(NEW_TOKENS), 1) - prefill) / (NEW_TOKENS - 1)
+        gens = lambda: [torch.Generator().manual_seed(i) for i in range(rows)]
+        seconds = caption_seconds(lambda: agent.generate_ids_batch(pxb, 0.2, 0.7, None, gens(), NEW_TOKENS))
+    return dict(rows=rows, prefill_ms=prefill, decode_ms_per_step=step_ms, seconds_per_call=seconds,
+                seconds_per_caption=[s / rows for s in seconds], gemv=bench_gemv_rows(rows))
+
+
+def caption_seconds(call, repeats=3):
+    """host seconds of `call` (which ends with the tokens on the host), after one warm-up call, `repeats` times"""
+    call()
+    torch.cuda.synchronize()
+    out = []
+    for _ in range(repeats):
+        t0 = time.perf_counter()
+        call()
+        torch.cuda.synchronize()
+        out.append(time.perf_counter() - t0)
+    return out
+
+
+def median(v):
+    return sorted(v)[len(v) // 2]
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--layers", type=int, default=40)
+    ap.add_argument("--rows", type=str, default=None, help="comma-separated row counts (1..8) of the batched decode")
     ap.add_argument("--json", type=str, default=None)
     args = ap.parse_args()
     from upscale_a_video_b200 import _lib
     _lib.load()
     res = dict(card=card(), layers=args.layers)
     print("card, power limit:", res["card"])
+    if args.rows:
+        agent = build_agent(args.layers)
+        agent.prompt_ids = lambda qs=None: [1] + list(range(100, 135)) + [-200] + list(range(200, 230))
+        agent.max_new_tokens = NEW_TOKENS
+        agent.eos_id = -1  # seeded weights: never stop early, every row decodes 64 tokens
+        px = torch.randn(3, 336, 336).half()
+        ids = agent.prompt_ids()
+        res["rows"] = []
+        for rows in map(int, args.rows.split(",")):
+            r = bench_rows(agent, px, ids, rows)
+            res["rows"].append(r)
+            for gv in r["gemv"]:
+                print(f"rows={rows} uav_gemv_rows N={gv['N']:6d} K={gv['K']:6d}: {gv['us']:8.1f} us  "
+                      f"{gv['GBs']:7.0f} GB/s  ({100 * gv['of_peak']:.0f}% of 3.35 TB/s)")
+            sc = r["seconds_per_call"]
+            print(f"rows={rows}: decode {r['decode_ms_per_step']:.2f} ms/step, prefill {r['prefill_ms']:.1f} ms, "
+                  f"{median(sc):.3f} s per call (median of {len(sc)}, {min(sc):.3f}-{max(sc):.3f}) = "
+                  f"{median(sc) / rows:.3f} s per caption")
+        if args.json:
+            json.dump(res, open(args.json, "w"), indent=1)
+        return
     res["gemv"] = bench_gemv()
     for r in res["gemv"]:
         print(f"uav_gemv N={r['N']:6d} K={r['K']:6d}: {r['us']:8.1f} us  {r['GBs']:7.0f} GB/s  "
@@ -111,30 +190,20 @@ def main():
         n = x.shape[0]
         steps = {}
 
-        def run(max_new):
-            for _ in agent._run(x, max_new, lambda step, logits: 29871):
-                pass
+        def run(max_new):  # prefill, then max_new - 1 decode steps
+            agent.forward_logits(x, [29871] * (max_new - 1))
 
         run(2)
         res["prefill_ms"] = events_ms(lambda: run(1), 3)  # prefill + lm_head of the last row
         t_all = events_ms(lambda: run(NEW_TOKENS), 2)
         res["ms_per_token"] = (t_all - res["prefill_ms"]) / (NEW_TOKENS - 1)
-        # a caption also reads each token back to the host
-        from upscale_a_video_b200 import ops
-        tok = torch.empty((), dtype=torch.int64, device="cuda")
-
-        def caption():
-            f = agent.vision_features(px)
-            xx = agent.embed_prompt(ids, f)
-            for _ in agent._run(xx, NEW_TOKENS, lambda s, lg: (int(ops.sample_top_p(lg, 0.2, 0.7, 0.5, out=tok)), tok)[1]):
-                pass
-
-        caption()
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        caption()
-        torch.cuda.synchronize()
-        res["seconds_per_caption"] = time.perf_counter() - t0
+        # a caption: vision tower, prefill and 64 sampled tokens, each read back to the host
+        agent.prompt_ids = lambda qs=None: ids
+        agent.eos_id = -1  # seeded weights: never stop early
+        sc = caption_seconds(lambda: agent.generate_ids(px, 0.2, 0.7, generator=torch.Generator().manual_seed(0),
+                                                        max_new_tokens=NEW_TOKENS))
+        res["seconds_per_caption"] = median(sc)
+        res["seconds_per_caption_runs"] = sc
         steps["n_prompt_rows"] = n
     res.update(steps)
     res["decode_GBs"] = weight_bytes / (res["ms_per_token"] * 1e-3) / 1e9

@@ -111,6 +111,10 @@ _PROTOS = {
     "uav_gemv": [P, I64, I64, P, P, P, I32, P],
     "uav_attention_decode": [P, P, P, I64, I64, I32, I32, F32, P, P, C.c_size_t, P],
     "uav_sample_top_p": [P, I64, F32, F32, F32, P, P],
+    "uav_gemv_rows": [P, I64, I64, P, I64, P, P, I32, P],
+    "uav_rope_kv_append_batched": [P, I64, I64, I64, I64, I32, I32, I64, P, I64, P, P, I64, I64, I64, P],
+    "uav_attention_decode_batched": [P, I64, P, P, I64, I64, I64, I64, I32, I32, F32, P, I64, P, C.c_size_t, P],
+    "uav_sample_top_p_batched": [P, I64, I64, I64, F32, F32, P, P, P],
 }
 _SPECIAL = {
     "uav_version": (C.c_char_p, []),
@@ -121,6 +125,7 @@ _SPECIAL = {
     "uav_plane_stats_workspace_bytes": (C.c_size_t, [I64]),
     "uav_instnorm_workspace_bytes": (C.c_size_t, [I64, I64]),
     "uav_attention_decode_workspace_bytes": (C.c_size_t, [I32, I64]),
+    "uav_attention_decode_batched_workspace_bytes": (C.c_size_t, [I64, I32, I64]),
 }
 
 

@@ -13,8 +13,10 @@ beyond the low-resolution sampling state.  Under `torchrun` (WORLD_SIZE > 1) eac
 and the pipeline's tile / window sharding splits the work; only rank 0 writes files.
 
 With `--llava_path` (and without `--no_llava`) frame 0 of each clip is captioned by `llava.LLavaAgent` before the
-upscale, with the reference's preprocessing and a generator seeded from SEED; the prompt is `caption + a_prompt`.  Under
-`torchrun` only rank 0 loads and runs the captioner and the caption is broadcast to the other ranks.
+upscale, with the reference's preprocessing and a generator seeded from SEED; the prompt is `caption + a_prompt`.  When
+clip i is reached and has no caption yet, the first frames of clips i .. i + CAPTION_BATCH - 1 are captioned in one
+call, each with its own generator seeded SEED, which gives each clip the caption a call on it alone gives.  Under
+`torchrun` only rank 0 loads and runs the captioner and the captions are broadcast to the other ranks.
 
 Deliberate differences from the reference CLI (INTEGRATION.md §3): the captioner runs only when `--llava_path` names a
 LLaVA-1.5 folder (otherwise `--caption` supplies the caption text), its sampling is seeded, errors raise instead of
@@ -99,15 +101,26 @@ def caption_frame(agent, frame_bgr: np.ndarray) -> str:
     return agent.gen_image_caption([img], generator=torch.Generator().manual_seed(SEED))[0]
 
 
-def _shared_caption(agent, frame_bgr, rank: int) -> str:
-    """rank 0 captions; under torch.distributed every rank gets its caption"""
+def caption_frames(agent, frames_bgr: List[np.ndarray]) -> List[str]:
+    """`caption_frame` of each frame, from one `gen_image_caption` call with one generator seeded SEED per frame"""
+    from .llava import frame0_image
+    imgs = [frame0_image(np.ascontiguousarray(f[..., ::-1])) for f in frames_bgr]
+    return agent.gen_image_caption(imgs, generator=[torch.Generator().manual_seed(SEED) for _ in imgs])
+
+
+def _shared_captions(agent, first_frame, video_paths: List[str], rank: int) -> List[str]:
+    """the captions of the clips `video_paths`, whose first clip's frame 0 is `first_frame`: rank 0 reads the other
+    clips' first frames and captions them all in one call; under torch.distributed every rank gets the list"""
     import torch.distributed as dist
-    caption = caption_frame(agent, frame_bgr) if rank == 0 else None
+    captions = None
+    if rank == 0:
+        frames = [first_frame] + [video_io.read_first_frame(p) for p in video_paths[1:]]
+        captions = caption_frames(agent, frames)
     if dist.is_initialized() and dist.get_world_size() > 1:
-        box = [caption]
+        box = [captions]
         dist.broadcast_object_list(box, src=0)
-        caption = box[0]
-    return caption
+        captions = box[0]
+    return captions
 
 
 def save_name(video_name: str, args: argparse.Namespace) -> str:
@@ -230,6 +243,8 @@ def main(argv: Optional[List[str]] = None) -> List[str]:
             from .llava import LLavaAgent
             log("Loading LLaVA")
             agent = LLavaAgent(args.llava_path, device=device, vision_tower_path=args.llava_vision_path)
+        from .llava import CAPTION_BATCH
+        captions: List[str] = []  # captions of the next clips, computed a group ahead
         written = []
         for i, video_path in enumerate(video_list):
             frames, fps, video_name = video_io.read_frames(video_path)
@@ -238,7 +253,9 @@ def main(argv: Optional[List[str]] = None) -> List[str]:
             caption = args.caption
             if use_llava(args):
                 log(f"{index_str} Generating video caption with LLaVA...")
-                caption = _shared_caption(agent, frames[0], rank)
+                if not captions:
+                    captions = _shared_captions(agent, frames[0], video_list[i:i + CAPTION_BATCH], rank)
+                caption = captions.pop(0)
                 log(textwrap.indent(textwrap.fill("Caption: " + caption, width=80), " " * 8))
             vframes = ingest_frames(frames, device, from_video=video_io.is_video(video_path))
             video_path_out, frame_dir = output_paths(args, video_name)

@@ -17,6 +17,9 @@ Path of one caption:
   append, causal attention; only the last row goes through lm_head;
 - decode, one token at a time: the same layers on one row with the GEMV weight stream and attention against the
   KV cache; the sampler picks the token on the device from one uniform drawn from `generator` on the host.
+Up to CAPTION_BATCH images go through this path together: one vision-tower batch, one prefill of B x n rows and one
+decode step for all B rows, so each decoded token streams the weights once for the whole batch.  Every kernel on the
+path gives each row the arithmetic of the one-row path, so a row's tokens do not depend on the rest of its batch.
 There is no CPU path."""
 from __future__ import annotations
 
@@ -33,7 +36,7 @@ from . import _lib, ops
 from .clip_text import encoder_layer
 
 __all__ = ["LLavaAgent", "IMAGE_TOKEN_INDEX", "conversation_prompt", "tokenize_prompt", "postprocess_caption",
-           "frame0_image", "clip_preprocess", "llava_key_map"]
+           "frame0_image", "clip_preprocess", "llava_key_map", "CAPTION_BATCH", "caption_groups"]
 
 IMAGE_TOKEN_INDEX = -200  # llava/constants.py
 DEFAULT_IMAGE_TOKEN = "<image>"
@@ -44,6 +47,7 @@ STOP_STR = "</s>"           # vicuna_v1's sep2
 MAX_NEW_TOKENS = 64         # llava_agent.py: generate(max_new_tokens=64)
 FRAME_SHORT_SIDE = 512      # inference_upscale_a_video.py: fix_resize
 PATCH_K_PADDED = 592        # 3 * 14 * 14 = 588 patch values, padded to a multiple of 16 for the GEMM
+CAPTION_BATCH = 8           # images per weight pass: the batched GEMV and sampler take up to 8 rows
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -240,6 +244,26 @@ def load_vision_tower(folder: str, vcfg: SimpleNamespace, layers: int, device) -
     return tower
 
 
+def caption_groups(n: int) -> List[range]:
+    """indices [0, n) in consecutive groups of at most CAPTION_BATCH, the batches `gen_image_caption` runs"""
+    return [range(i, min(i + CAPTION_BATCH, n)) for i in range(0, n, CAPTION_BATCH)]
+
+
+def _caption_generators(n: int, temperature: float, generator):
+    """(one generator per image, whether the images may share a batch).  A list of distinct generators gives each
+    image its own uniforms, drawn as a one-image call draws them, so batching cannot change them; greedy decoding
+    draws none.  A generator shared by several images (a single generator, None for the global RNG, or one object
+    listed twice) at temperature > 0 is drawn across those images in the one-at-a-time loop's order, which only that
+    loop reproduces."""
+    if isinstance(generator, (list, tuple)):
+        if len(generator) != n:
+            raise ValueError(f"generator: a list of {len(generator)} generators for {n} images; pass one per image")
+        gens = list(generator)
+        distinct = None not in gens and len({id(g) for g in gens}) == n
+        return gens, temperature == 0 or distinct
+    return [generator] * n, temperature == 0
+
+
 # ---------------------------------------------------------------------------------------------------------------
 # the agent
 # ---------------------------------------------------------------------------------------------------------------
@@ -329,29 +353,43 @@ class LLavaAgent:
     @torch.no_grad()
     def vision_features(self, pixel_values: torch.Tensor) -> torch.Tensor:
         """(3, S, S) preprocessed image (host or device) -> (patches, mm_hidden_size) fp16 features of the selected layer,
-        CLS dropped"""
+        CLS dropped; (B, 3, S, S) images -> (B, patches, mm_hidden_size), the encoder layers run on all B at once"""
         vc, t = self.vision_config, self.tower
         ps = vc.patch_size
         g = vc.image_size // ps
         px = pixel_values.to(torch.float16).cpu()
-        assert px.shape == (3, vc.image_size, vc.image_size), px.shape
-        patches = px.view(3, g, ps, g, ps).permute(1, 3, 0, 2, 4).reshape(g * g, 3 * ps * ps)
+        one = px.dim() == 3
+        px = px[None] if one else px
+        B = px.shape[0]
+        assert px.shape[1:] == (3, vc.image_size, vc.image_size), px.shape
+        patches = px.view(B, 3, g, ps, g, ps).permute(0, 2, 4, 1, 3, 5).reshape(B * g * g, 3 * ps * ps)
         patches = F.pad(patches, (0, PATCH_K_PADDED - patches.shape[1])).to(self.device)
-        emb = ops.linear(patches, t.patch_w)
-        x = (torch.cat([t.cls[None], emb]).float() + t.pos.float()).to(torch.float16)[None]  # one rounding
+        emb = ops.linear(patches, t.patch_w).view(B, g * g, -1)
+        cls = t.cls[None, None].expand(B, 1, -1)
+        x = (torch.cat([cls, emb], 1).float() + t.pos.float()).to(torch.float16)  # one rounding
         x = ops.layer_norm(x, *t.pre_ln, vc.layer_norm_eps)
         act = ops.ACT_GELU if vc.hidden_act == "gelu" else ops.ACT_QUICK_GELU
         for w in t.layers:
             x = encoder_layer(x, w, vc.num_attention_heads, vc.layer_norm_eps, act, causal=False)
-        return x[0, 1:]
+        return x[0, 1:] if one else x[:, 1:]
 
+    # The layers take B sequences: x holds B x n prefill rows (sequence-major) or B decode rows, and the caches are
+    # (B, L_max, hidden) (or (L_max, hidden) for B = 1).  The prefill GEMMs run on all B x n rows: uav_linear picks its
+    # tile width from N alone for a single-tap GEMM without GEGLU, so each output element's k-order does not depend on
+    # M, and a sequence's rows come out as they do in a prefill of that sequence alone.
     def _layer_prefill(self, i, x, kc, vc_, rope):
         cfg, w = self.config, self.w
         H, heads, eps = cfg.hidden_size, cfg.num_attention_heads, cfg.rms_norm_eps
-        n = x.shape[0]
+        if kc.dim() == 2:
+            kc, vc_ = kc[None], vc_[None]
+        B = kc.shape[0]
+        n = x.shape[0] // B
         qkv = ops.linear(ops.rms_norm(x, w[f"ln1_{i}"], eps), w[f"qkv{i}"])
-        ops.rope_kv_append(qkv, heads, 0, rope, kc, vc_)
-        o = ops.attention_causal(qkv[:, :H].unsqueeze(0), kc[:n].unsqueeze(0), vc_[:n].unsqueeze(0), heads)[0]
+        ops.rope_kv_append_batched(qkv.view(B, n, -1), heads, 0, rope, kc, vc_)
+        o = torch.empty(B * n, H, dtype=torch.float16, device=x.device)
+        for b in range(B):  # the causal kernel reads a batch's keys n rows apart; each cache is L_max rows long
+            ops.attention_causal(qkv[b * n:(b + 1) * n, :H].unsqueeze(0), kc[b, :n].unsqueeze(0),
+                                 vc_[b, :n].unsqueeze(0), heads, out=o[b * n:(b + 1) * n].unsqueeze(0))
         x = ops.linear(o, w[f"o{i}"], residual=x)
         gu = ops.linear(ops.rms_norm(x, w[f"ln2_{i}"], eps), w[f"gu{i}"])
         return ops.linear(ops.swiglu(gu), w[f"down{i}"], residual=x)
@@ -359,16 +397,20 @@ class LLavaAgent:
     def _layer_decode(self, i, x, pos, kc, vc_, rope):
         cfg, w = self.config, self.w
         H, heads, eps = cfg.hidden_size, cfg.num_attention_heads, cfg.rms_norm_eps
-        qkv = ops.gemv(w[f"qkv{i}"], ops.rms_norm(x, w[f"ln1_{i}"], eps))
-        ops.rope_kv_append(qkv.view(1, -1), heads, pos, rope, kc, vc_)
-        o = ops.attention_decode(qkv[:H], kc, vc_, pos + 1, heads)
-        x = ops.gemv(w[f"o{i}"], o, residual=x).view(1, H)
-        gu = ops.gemv(w[f"gu{i}"], ops.rms_norm(x, w[f"ln2_{i}"], eps))
-        return ops.gemv(w[f"down{i}"], ops.swiglu(gu.view(1, -1)), residual=x).view(1, H)
+        if kc.dim() == 2:
+            kc, vc_ = kc[None], vc_[None]
+        B = x.shape[0]
+        qkv = ops.gemv_rows(w[f"qkv{i}"], ops.rms_norm(x, w[f"ln1_{i}"], eps))
+        ops.rope_kv_append_batched(qkv.view(B, 1, -1), heads, pos, rope, kc, vc_)
+        o = ops.attention_decode_batched(qkv[:, :H], kc, vc_, pos + 1, heads)
+        x = ops.gemv_rows(w[f"o{i}"], o, residual=x)
+        gu = ops.gemv_rows(w[f"gu{i}"], ops.rms_norm(x, w[f"ln2_{i}"], eps))
+        return ops.gemv_rows(w[f"down{i}"], ops.swiglu(gu), residual=x)
 
-    def _logits(self, x_row):
-        h = ops.rms_norm(x_row, self.w["norm"], self.config.rms_norm_eps)
-        return ops.gemv(self.w["lm_head"], h, out_dtype=torch.float32)
+    def _logits(self, x_rows):
+        """fp32 (B, vocab) logits of the rows x_rows (B, hidden) (a strided row view allowed)"""
+        h = ops.rms_norm(x_rows, self.w["norm"], self.config.rms_norm_eps)
+        return ops.gemv_rows(self.w["lm_head"], h, out_dtype=torch.float32)
 
     def prompt_ids(self, qs: Optional[str] = None) -> List[int]:
         prompt = conversation_prompt(self.qs if qs is None else qs)
@@ -377,43 +419,63 @@ class LLavaAgent:
     @torch.no_grad()
     def embed_prompt(self, ids: List[int], features: torch.Tensor) -> torch.Tensor:
         """(n, hidden) fp16 prefill rows: token embeddings, with the `IMAGE_TOKEN_INDEX` placeholder replaced by the
-        projected image features (the projector's second GEMM writes into those rows)"""
+        projected image features (the projector's second GEMM writes into those rows).  Features of B images
+        (B, patches, mm_hidden_size) give (B, n, hidden)."""
         w, H = self.w, self.config.hidden_size
+        one = features.dim() == 2
+        feats = features[None] if one else features
+        B, n_img = feats.shape[:2]
         at = ids.index(IMAGE_TOKEN_INDEX)
-        n_img = features.shape[0]
         text = torch.tensor(ids[:at] + ids[at + 1:], dtype=torch.int64, device=self.device)
         tok = w["embed"].index_select(0, text)
-        x = torch.empty(len(ids) - 1 + n_img, H, dtype=torch.float16, device=self.device)
-        x[:at] = tok[:at]
-        x[at + n_img:] = tok[at:]
-        h = ops.linear(features, w["proj0_w"], w["proj0_b"], act=ops.ACT_GELU)
-        ops.linear(h, w["proj2_w"], w["proj2_b"], out=x[at:at + n_img])
-        return x
+        x = torch.empty(B, len(ids) - 1 + n_img, H, dtype=torch.float16, device=self.device)
+        x[:, :at] = tok[:at]
+        x[:, at + n_img:] = tok[at:]
+        h = ops.linear(feats.reshape(B * n_img, -1), w["proj0_w"], w["proj0_b"], act=ops.ACT_GELU)
+        for b in range(B):
+            ops.linear(h[b * n_img:(b + 1) * n_img], w["proj2_w"], w["proj2_b"], out=x[b, at:at + n_img])
+        return x[0] if one else x
 
     @torch.no_grad()
     def forward_logits(self, x: torch.Tensor, forced: List[int]) -> List[torch.Tensor]:
-        """fp32 logits of the last prefill row of `x` (n, hidden), then of each decode step fed the tokens `forced`
-        (teacher forcing)"""
-        return list(self._run(x, len(forced) + 1, lambda step, logits: forced[step] if step < len(forced) else None))
+        """fp32 logits (vocab,) of the last prefill row of `x` (n, hidden), then of each decode step fed the tokens
+        `forced` (teacher forcing): `forward_logits_batch` of one sequence"""
+        return [logits[0] for logits in self.forward_logits_batch(x[None], [forced])]
+
+    @torch.no_grad()
+    def forward_logits_batch(self, x: torch.Tensor, forced: List[List[int]]) -> List[torch.Tensor]:
+        """fp32 logits (B, vocab) of the last prefill row of each sequence of `x` (B, n, hidden), then of each decode
+        step, row b fed the tokens forced[b] (teacher forcing; every row forces the same number of tokens)"""
+        B = x.shape[0]
+        steps = len(forced[0])
+        assert len(forced) == B and all(len(f) == steps for f in forced), "one list of forced tokens per row, equal lengths"
+
+        def pick(step, logits):
+            if step >= steps:
+                return None
+            return torch.tensor([f[step] for f in forced], dtype=torch.int64, device=self.device)
+
+        with torch.cuda.device(self.device):
+            return list(self._run(x, steps + 1, pick))
 
     def _run(self, x, max_new, pick):
-        """prefill x, then decode; pick(step, logits) -> a token id (int or device scalar) or None to stop; yields the
-        logits of every step"""
+        """prefill x (B, n, hidden), then decode the B sequences together; pick(step, logits) -> device int64 (B,)
+        token ids or None to stop; yields the fp32 (B, vocab) logits of every step"""
         cfg = self.config
-        n, L = x.shape[0], x.shape[0] + max_new
-        cache = torch.empty(cfg.num_hidden_layers, 2, L, cfg.hidden_size, dtype=torch.float16, device=self.device)
+        B, n, H = x.shape
+        L = n + max_new
+        cache = torch.empty(cfg.num_hidden_layers, 2, B, L, H, dtype=torch.float16, device=self.device)
         rope = self._rope_table(L)
+        x = x.reshape(B * n, H)
         for i in range(cfg.num_hidden_layers):
             x = self._layer_prefill(i, x, cache[i, 0], cache[i, 1], rope)
-        logits = self._logits(x[n - 1:n])
+        logits = self._logits(x.view(B, n, H)[:, n - 1])
         for step in range(max_new):
             yield logits
             tok = pick(step, logits)
             if tok is None or step == max_new - 1:
                 return
-            if not torch.is_tensor(tok):
-                tok = torch.tensor(tok, dtype=torch.int64, device=self.device)
-            xr = self.w["embed"].index_select(0, tok.view(1))
+            xr = self.w["embed"].index_select(0, tok.view(B))
             for i in range(cfg.num_hidden_layers):
                 xr = self._layer_decode(i, xr, n + step, cache[i, 0], cache[i, 1], rope)
             logits = self._logits(xr)
@@ -422,21 +484,46 @@ class LLavaAgent:
     def generate_ids(self, pixel_values: torch.Tensor, temperature=0.2, top_p=0.7, qs=None, generator=None,
                      max_new_tokens: Optional[int] = None) -> List[int]:
         """the new token ids (EOS included when reached) for one preprocessed image"""
+        return self.generate_ids_batch(pixel_values[None], temperature, top_p, qs, [generator], max_new_tokens)[0]
+
+    @torch.no_grad()
+    def generate_ids_batch(self, pixel_values: torch.Tensor, temperature=0.2, top_p=0.7, qs=None, generators=None,
+                           max_new_tokens: Optional[int] = None) -> List[List[int]]:
+        """the new token ids (EOS included when reached) of each of B <= CAPTION_BATCH preprocessed images
+        (B, 3, S, S), decoded together.  Row b draws one uniform per token from generators[b] (None: the global RNG)
+        until it emits EOS, as `generate_ids` of that image alone does; a finished row is fed EOS and its outputs are
+        ignored.  Decoding ends when every row has finished or after max_new_tokens."""
+        B = pixel_values.shape[0]
+        assert 1 <= B <= CAPTION_BATCH, B
+        generators = [None] * B if generators is None else list(generators)
+        assert len(generators) == B
         ids = self.prompt_ids(qs)
+        out: List[List[int]] = [[] for _ in range(B)]
+        done = [False] * B
         with torch.cuda.device(self.device):
             x = self.embed_prompt(ids, self.vision_features(pixel_values))
-            out: List[int] = []
-            tok_buf = torch.empty((), dtype=torch.int64, device=self.device)
+            tok_buf = torch.empty(B, dtype=torch.int64, device=self.device)
 
             def pick(step, logits):
-                u = 0.0
-                if temperature > 0:
-                    gdev = generator.device if generator is not None else "cpu"
-                    u = float(torch.rand((), generator=generator, device=gdev, dtype=torch.float64).item())
-                tok = ops.sample_top_p(logits, float(temperature), float(top_p), min(u, 1.0 - 2 ** -24), out=tok_buf)
-                t = int(tok.item())  # the host reads each token back once, to stop at EOS
-                out.append(t)
-                return None if t == self.eos_id else tok
+                us = []
+                for b, g in enumerate(generators):
+                    u = 0.0
+                    if temperature > 0 and not done[b]:
+                        gdev = g.device if g is not None else "cpu"
+                        u = float(torch.rand((), generator=g, device=gdev, dtype=torch.float64).item())
+                    us.append(min(u, 1.0 - 2 ** -24))
+                tok = ops.sample_top_p_batched(logits, float(temperature), float(top_p), us, out=tok_buf)
+                toks = tok.tolist()  # the host reads the B tokens back once per step, to stop at EOS
+                for b, t in enumerate(toks):
+                    if not done[b]:
+                        out[b].append(t)
+                        done[b] = t == self.eos_id
+                if all(done):
+                    return None
+                if any(done):
+                    return torch.tensor([self.eos_id if d else t for d, t in zip(done, toks)], dtype=torch.int64,
+                                        device=self.device)
+                return tok
 
             for _ in self._run(x, max_new_tokens or self.max_new_tokens, pick):
                 pass
@@ -447,13 +534,20 @@ class LLavaAgent:
         return self.sp.decode([i for i in ids if i not in self.special_ids])
 
     def gen_image_caption(self, imgs, temperature=0.2, top_p=0.7, num_beams=1, qs=None, *, generator=None):
-        """one caption per PIL image, as the reference's agent returns them"""
+        """one caption per PIL image, as the reference's agent returns them.  `generator` is one torch.Generator for
+        all images, or a list of one per image; None draws from the global RNG.  The images are decoded in batches of
+        up to CAPTION_BATCH when that gives the captions of one-image calls: greedily (temperature 0) or with a
+        list of distinct generators.  A generator shared between images (a single one, None, or one object listed
+        twice) at temperature > 0 captions the images one at a time."""
         if num_beams != 1:
             raise NotImplementedError("beam search (num_beams > 1) is not supported")
         if temperature < 0:
             raise ValueError("temperature must be >= 0")
+        gens, batched = _caption_generators(len(imgs), temperature, generator)
+        groups = caption_groups(len(imgs)) if batched else [range(i, i + 1) for i in range(len(imgs))]
         caps = []
-        for img in imgs:
-            ids = self.generate_ids(clip_preprocess(img, self.image_processor), temperature, top_p, qs, generator)
-            caps.append(postprocess_caption(self.decode(ids)))
+        for group in groups:
+            px = torch.stack([clip_preprocess(imgs[i], self.image_processor) for i in group])
+            for ids in self.generate_ids_batch(px, temperature, top_p, qs, [gens[i] for i in group]):
+                caps.append(postprocess_caption(self.decode(ids)))
         return caps

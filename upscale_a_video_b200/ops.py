@@ -999,3 +999,80 @@ def sample_top_p(logits: torch.Tensor, temperature: float, top_p: float, u: floa
     _lib.check(_lib.load().uav_sample_top_p(logits.data_ptr(), logits.numel(), temperature, top_p, u, out.data_ptr(),
                                             _stream()), "uav_sample_top_p")
     return out
+
+
+# batched decode: B sequences per step (llava.py captions up to 8 images per weight pass); each row's result is
+# bit-identical to the one-row op on that row
+def gemv_rows(w: torch.Tensor, x: torch.Tensor, *, residual=None, out=None, out_dtype=torch.float16):
+    """out (rows, N) = x (rows, K) @ w (N, K)^T (+ residual (rows, N)), 1 <= rows <= 8, w streamed once for all rows"""
+    assert w.is_cuda and w.dtype == torch.float16 and w.is_contiguous() and w.dim() == 2
+    N, K = w.shape
+    assert x.dtype == torch.float16 and x.dim() == 2 and x.shape[1] == K and x.is_contiguous()
+    rows = x.shape[0]
+    assert 1 <= rows <= 8, rows
+    if out is None:
+        out = torch.empty(rows, N, dtype=out_dtype, device=w.device)
+    assert out.shape == (rows, N) and out.is_contiguous() and out.dtype in (torch.float16, torch.float32)
+    if residual is not None:
+        assert residual.dtype == torch.float16 and residual.shape == (rows, N) and residual.is_contiguous()
+    with _timed("gemv", 2.0 * rows * N * K, 2.0 * (N * K + rows * (K + N)), f"gemv_rows{rows} N{N} K{K}"):
+        _lib.check(_lib.load().uav_gemv_rows(w.data_ptr(), N, K, x.data_ptr(), rows,
+                                             0 if residual is None else residual.data_ptr(), out.data_ptr(),
+                                             F16 if out.dtype == torch.float16 else F32, _stream()),
+                   "uav_gemv_rows")
+    return out
+
+
+def _batched_cache(k_cache: torch.Tensor, v_cache: torch.Tensor):
+    """(batch, rows, batch stride, row stride) of per-sequence KV caches (B, L_max, heads 128) fp16"""
+    assert k_cache.is_cuda and k_cache.dtype == torch.float16 and k_cache.dim() == 3 and k_cache.stride(-1) == 1
+    assert v_cache.shape == k_cache.shape and v_cache.stride() == k_cache.stride() and v_cache.dtype == torch.float16
+    return k_cache.shape[0], k_cache.shape[1], k_cache.stride(0), k_cache.stride(1)
+
+
+def rope_kv_append_batched(qkv: torch.Tensor, heads: int, p0: int, cos_sin: torch.Tensor, k_cache: torch.Tensor,
+                           v_cache: torch.Tensor):
+    """rope_kv_append on B sequences: qkv (B, n, >= 3 heads 128) fused q|k|v rows at positions [p0, p0 + n) of every
+    sequence (q rotated in place); k_cache / v_cache (B, L_max, heads 128)"""
+    assert qkv.is_cuda and qkv.dtype == torch.float16 and qkv.dim() == 3 and qkv.stride(-1) == 1
+    B, n, _ = qkv.shape
+    Bc, rows, kv_bs, ld_kv = _batched_cache(k_cache, v_cache)
+    assert Bc == B, (Bc, B)
+    assert cos_sin.dtype == torch.float32 and cos_sin.is_contiguous() and cos_sin.shape[1:] == (64, 2)
+    _lib.check(_lib.load().uav_rope_kv_append_batched(qkv.data_ptr(), qkv.stride(1), qkv.stride(0), B, n, heads, 128,
+                                                      p0, cos_sin.data_ptr(), cos_sin.shape[0], k_cache.data_ptr(),
+                                                      v_cache.data_ptr(), ld_kv, kv_bs, rows, _stream()),
+               "uav_rope_kv_append_batched")
+
+
+def attention_decode_batched(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, L: int, heads: int, *,
+                             scale: Optional[float] = None, out=None):
+    """attention_decode on B sequences: q (B, heads 128) fp16 (a column slice of the fused q|k|v rows allowed)
+    against rows [0, L) of each sequence's cache (B, L_max, heads 128) -> (B, heads 128) fp16"""
+    B, _, kv_bs, ld_kv = _batched_cache(k_cache, v_cache)
+    assert q.is_cuda and q.dtype == torch.float16 and q.shape == (B, heads * 128) and q.stride(-1) == 1
+    if out is None:
+        out = torch.empty(B, heads * 128, dtype=torch.float16, device=q.device)
+    assert out.dtype == torch.float16 and out.shape == (B, heads * 128) and out.stride(-1) == 1
+    lib = _lib.load()
+    ws_bytes = int(lib.uav_attention_decode_batched_workspace_bytes(B, heads, L))
+    ws = torch.empty(ws_bytes // 4, dtype=torch.float32, device=q.device)
+    _lib.check(lib.uav_attention_decode_batched(q.data_ptr(), q.stride(0), k_cache.data_ptr(), v_cache.data_ptr(),
+                                                ld_kv, kv_bs, B, L, heads, 128, 128 ** -0.5 if scale is None else scale,
+                                                out.data_ptr(), out.stride(0), ws.data_ptr(), ws_bytes, _stream()),
+               "uav_attention_decode_batched")
+    return out
+
+
+def sample_top_p_batched(logits: torch.Tensor, temperature: float, top_p: float, u, out=None) -> torch.Tensor:
+    """sample_top_p on each row of fp32 logits (B, V), B <= 8, row b at uniform u[b] -> (B,) device int64 tokens"""
+    assert logits.is_cuda and logits.dtype == torch.float32 and logits.dim() == 2 and logits.stride(-1) == 1
+    B, V = logits.shape
+    assert 1 <= B <= 8 and len(u) == B, (B, len(u))
+    if out is None:
+        out = torch.empty(B, dtype=torch.int64, device=logits.device)
+    assert out.dtype == torch.int64 and out.shape == (B,) and out.is_contiguous()
+    us = (C.c_float * B)(*u)
+    _lib.check(_lib.load().uav_sample_top_p_batched(logits.data_ptr(), logits.stride(0), B, V, temperature, top_p, us,
+                                                    out.data_ptr(), _stream()), "uav_sample_top_p_batched")
+    return out

@@ -95,6 +95,27 @@ def read_frames(path: str) -> Tuple[np.ndarray, Optional[float], str]:
     return np.stack(frames), fps, name
 
 
+def read_first_frame(path: str) -> np.ndarray:
+    """frame 0 of a clip, (h, w, 3) uint8 BGR, equal to `read_frames(path)[0][0]` without reading the other frames"""
+    cv2 = _cv2()
+    if is_video(path):
+        cap = cv2.VideoCapture(path)
+        if not cap.isOpened():
+            raise RuntimeError(f"OpenCV cannot open the video {path}")
+        ok, frame = cap.read()
+        cap.release()
+        if not ok:
+            raise RuntimeError(f"no frames in {path}")
+        return frame
+    for f in sorted(os.listdir(path)):
+        if is_image(f):
+            frame = cv2.imread(os.path.join(path, f), cv2.IMREAD_COLOR)
+            if frame is None:
+                raise RuntimeError(f"OpenCV cannot read the image {os.path.join(path, f)}")
+            return frame
+    raise RuntimeError(f"no frames in {path}")
+
+
 class VideoWriter:
     """mp4 (fourcc mp4v) written chunk by chunk: opened once for frames of (h, w), then `write((t, h, w, 3) uint8 RGB)`
     per chunk; fps None -> DEFAULT_FPS.  A context manager: the file is finalised when the block ends."""
