@@ -5,10 +5,13 @@ importable, `LlamaForCausalLM.generate` (fp16, greedy, 64 new tokens) on the sam
 baseline.  Prints the card's name and power limit first.
 
 With `--rows 1,2,4,8`, for each row count B: `uav_gemv_rows` µs and GB/s at the five decode shapes, ms per batched
-decode step (B rows, one weight pass), and seconds for one `generate_ids_batch` call captioning B images (vision tower,
-prefill, 64 sampled tokens per row).
+decode step (B rows, one weight pass), the prefill's ms, and seconds for one `generate_ids_batch` call captioning B
+images (vision tower, prefill, 64 sampled tokens per row).  `--weights fp16,int8` builds one agent per weight format
+(the int8 one quantizes each seeded matrix as it is made, so no fp16 copy of it is held), reports each agent's
+`memory_allocated()`, and times the formats alternately for each row count; the int8 decoder shapes are timed on
+`uav_gemv_rows_int8`, whose bytes are N K + 4 N + 2 B (K + N).
 
-    python tools/bench_llava.py [--layers 40] [--rows 1,2,4,8] [--json out.json]
+    python tools/bench_llava.py [--layers 40] [--rows 1,2,4,8] [--weights fp16,int8] [--json out.json]
 """
 import argparse
 import json
@@ -44,27 +47,38 @@ def events_ms(fn, iters):
     return s.elapsed_time(e) / iters
 
 
-def build_agent(layers: int):
-    from upscale_a_video_b200.llava import PATCH_K_PADDED, LLavaAgent
+def build_agent(layers: int, weights: str = "fp16"):
+    from upscale_a_video_b200 import ops
+    from upscale_a_video_b200.llava import PATCH_K_PADDED, Int8Rows, LLavaAgent, dequant_scratch
     g = torch.Generator(device="cuda").manual_seed(0)
     lin = lambda a, b, s=1.0: (torch.randn(a, b, generator=g, device="cuda", dtype=torch.float16) * (s / b ** 0.5))
+    if weights == "int8":
+        lin16 = lin
+
+        def lin(a, b, s=1.0):  # the agent's int8 Linears, quantized as they are made
+            t = Int8Rows(torch.empty(a, b, dtype=torch.int8, device="cuda"),
+                         torch.empty(a, dtype=torch.float32, device="cuda"))
+            ops.quantize_rows_int8(lin16(a, b, s), t.q, t.absmax)
+            return t
     vec = lambda n, c=1.0: (c + 0.1 * torch.randn(n, generator=g, device="cuda")).half()
     agent = LLavaAgent.__new__(LLavaAgent)
     agent.device = torch.device("cuda", torch.cuda.current_device())
     agent.config = SimpleNamespace(hidden_size=H, num_attention_heads=HEADS, num_hidden_layers=layers, rms_norm_eps=1e-5,
                                    rope_theta=10000.0, vocab_size=VOCAB)
-    w = {"embed": lin(VOCAB, H, H ** 0.5 * 0.02), "norm": vec(H), "lm_head": lin(VOCAB, H, 3.0),
+    lin_fp16 = lin16 if weights == "int8" else lin
+    w = {"embed": lin_fp16(VOCAB, H, H ** 0.5 * 0.02), "norm": vec(H), "lm_head": lin_fp16(VOCAB, H, 3.0),
          "proj0_w": lin(H, VH), "proj0_b": torch.zeros(H, device="cuda"), "proj2_w": lin(H, H),
          "proj2_b": torch.zeros(H, device="cuda")}
     for i in range(layers):
         w.update({f"qkv{i}": lin(3 * H, H), f"o{i}": lin(H, H), f"gu{i}": lin(2 * INTER, H), f"down{i}": lin(H, INTER),
                   f"ln1_{i}": vec(H), f"ln2_{i}": vec(H)})
     agent.w = w
+    agent._dq = dequant_scratch(w, agent.device)
     f32 = lambda n, c=0.0: (c + 0.02 * torch.randn(n, generator=g, device="cuda")).float()
-    vl = lambda a, b: (lin(a, b), f32(a))
+    vl = lambda a, b: (lin_fp16(a, b), f32(a))
     agent.vision_config = SimpleNamespace(hidden_size=VH, num_attention_heads=VHEADS, image_size=336, patch_size=14,
                                           hidden_act="quick_gelu", layer_norm_eps=1e-5)
-    agent.tower = SimpleNamespace(patch_w=lin(VH, PATCH_K_PADDED), cls=vec(VH, 0.0), pos=vec(577 * VH, 0.0).view(577, VH),
+    agent.tower = SimpleNamespace(patch_w=lin_fp16(VH, PATCH_K_PADDED), cls=vec(VH, 0.0), pos=vec(577 * VH, 0.0).view(577, VH),
                                   pre_ln=(f32(VH, 1.0), f32(VH)), layers=[
                                       SimpleNamespace(ln1=(f32(VH, 1.0), f32(VH)), qkv=vl(3 * VH, VH), out=vl(VH, VH),
                                                       ln2=(f32(VH, 1.0), f32(VH)), fc1=vl(VINTER, VH), fc2=vl(VH, VINTER))
@@ -89,23 +103,33 @@ def bench_gemv():
     return rows
 
 
-def bench_gemv_rows(rows):
+def bench_gemv_rows(rows, weights="fp16"):
+    """µs and GB/s of the decode GEMV per shape; with int8 weights the decoder shapes run `uav_gemv_rows_int8` and
+    lm_head (fp16 in both formats) `uav_gemv_rows`"""
     from upscale_a_video_b200 import ops
     out_rows = []
     for N, K in ((3 * H, H), (H, H), (2 * INTER, H), (H, INTER), (VOCAB, H)):
         w = torch.randn(N, K, device="cuda", dtype=torch.float16)
         x = torch.randn(rows, K, device="cuda", dtype=torch.float16)
         out = torch.empty(rows, N, device="cuda", dtype=torch.float16)
+        if weights == "int8" and N != VOCAB:
+            q, s = torch.empty(N, K, dtype=torch.int8, device="cuda"), torch.empty(N, device="cuda")
+            ops.quantize_rows_int8(w, q, s)
+            call = lambda: ops.gemv_rows_int8(q, s, x, out=out)
+            nbytes = N * K + 4 * N + 2 * rows * (K + N)
+        else:
+            call = lambda: ops.gemv_rows(w, x, out=out)
+            nbytes = N * K * 2
         for _ in range(5):
-            ops.gemv_rows(w, x, out=out)
-        ms = events_ms(lambda: ops.gemv_rows(w, x, out=out), 200)
-        gbs = N * K * 2 / (ms * 1e-3) / 1e9
-        out_rows.append(dict(N=N, K=K, us=ms * 1e3, GBs=gbs, of_peak=gbs / (HBM_TBS * 1e3)))
-        del w
+            call()
+        ms = events_ms(call, 200)
+        gbs = nbytes / (ms * 1e-3) / 1e9
+        out_rows.append(dict(N=N, K=K, weights=weights, us=ms * 1e3, GBs=gbs, of_peak=gbs / (HBM_TBS * 1e3)))
+        del w, call
     return out_rows
 
 
-def bench_rows(agent, px, ids, rows):
+def bench_rows(agent, px, ids, rows, weights="fp16"):
     """decode ms per step of `rows` sequences and seconds of one caption call on `rows` images"""
     pxb = px[None].expand(rows, -1, -1, -1).contiguous()
     with torch.no_grad():
@@ -121,8 +145,8 @@ def bench_rows(agent, px, ids, rows):
         step_ms = (events_ms(lambda: run(NEW_TOKENS), 1) - prefill) / (NEW_TOKENS - 1)
         gens = lambda: [torch.Generator().manual_seed(i) for i in range(rows)]
         seconds = caption_seconds(lambda: agent.generate_ids_batch(pxb, 0.2, 0.7, None, gens(), NEW_TOKENS))
-    return dict(rows=rows, prefill_ms=prefill, decode_ms_per_step=step_ms, seconds_per_call=seconds,
-                seconds_per_caption=[s / rows for s in seconds], gemv=bench_gemv_rows(rows))
+    return dict(rows=rows, weights=weights, prefill_ms=prefill, decode_ms_per_step=step_ms, seconds_per_call=seconds,
+                seconds_per_caption=[s / rows for s in seconds], gemv=bench_gemv_rows(rows, weights))
 
 
 def caption_seconds(call, repeats=3):
@@ -146,6 +170,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--layers", type=int, default=40)
     ap.add_argument("--rows", type=str, default=None, help="comma-separated row counts (1..8) of the batched decode")
+    ap.add_argument("--weights", type=str, default="fp16",
+                    help="comma-separated weight formats of the --rows mode (fp16, int8), timed alternately")
     ap.add_argument("--json", type=str, default=None)
     args = ap.parse_args()
     from upscale_a_video_b200 import _lib
@@ -153,23 +179,36 @@ def main():
     res = dict(card=card(), layers=args.layers)
     print("card, power limit:", res["card"])
     if args.rows:
-        agent = build_agent(args.layers)
-        agent.prompt_ids = lambda qs=None: [1] + list(range(100, 135)) + [-200] + list(range(200, 230))
-        agent.max_new_tokens = NEW_TOKENS
-        agent.eos_id = -1  # seeded weights: never stop early, every row decodes 64 tokens
+        formats = args.weights.split(",")
+        assert all(f in ("fp16", "int8") for f in formats), formats
+        agents = {}
+        res["agent_bytes"] = {}
+        for f in formats:
+            torch.cuda.synchronize()
+            before = torch.cuda.memory_allocated()
+            agent = build_agent(args.layers, f)
+            torch.cuda.synchronize()
+            res["agent_bytes"][f] = torch.cuda.memory_allocated() - before
+            print(f"{f} agent: memory_allocated() {res['agent_bytes'][f] / 1e9:.2f} GB ({args.layers} layers)")
+            agent.prompt_ids = lambda qs=None: [1] + list(range(100, 135)) + [-200] + list(range(200, 230))
+            agent.max_new_tokens = NEW_TOKENS
+            agent.eos_id = -1  # seeded weights: never stop early, every row decodes 64 tokens
+            agents[f] = agent
         px = torch.randn(3, 336, 336).half()
-        ids = agent.prompt_ids()
+        ids = agents[formats[0]].prompt_ids()
         res["rows"] = []
         for rows in map(int, args.rows.split(",")):
-            r = bench_rows(agent, px, ids, rows)
-            res["rows"].append(r)
-            for gv in r["gemv"]:
-                print(f"rows={rows} uav_gemv_rows N={gv['N']:6d} K={gv['K']:6d}: {gv['us']:8.1f} us  "
-                      f"{gv['GBs']:7.0f} GB/s  ({100 * gv['of_peak']:.0f}% of 3.35 TB/s)")
-            sc = r["seconds_per_call"]
-            print(f"rows={rows}: decode {r['decode_ms_per_step']:.2f} ms/step, prefill {r['prefill_ms']:.1f} ms, "
-                  f"{median(sc):.3f} s per call (median of {len(sc)}, {min(sc):.3f}-{max(sc):.3f}) = "
-                  f"{median(sc) / rows:.3f} s per caption")
+            for f in formats:
+                r = bench_rows(agents[f], px, ids, rows, f)
+                res["rows"].append(r)
+                for gv in r["gemv"]:
+                    kernel = "uav_gemv_rows_int8" if f == "int8" and gv["N"] != VOCAB else "uav_gemv_rows"
+                    print(f"rows={rows} {f} {kernel:18s} N={gv['N']:6d} K={gv['K']:6d}: {gv['us']:8.1f} us  "
+                          f"{gv['GBs']:7.0f} GB/s  ({100 * gv['of_peak']:.0f}% of 3.35 TB/s)")
+                sc = r["seconds_per_call"]
+                print(f"rows={rows} {f}: decode {r['decode_ms_per_step']:.2f} ms/step, prefill {r['prefill_ms']:.1f} ms, "
+                      f"{median(sc):.3f} s per call (median of {len(sc)}, {min(sc):.3f}-{max(sc):.3f}) = "
+                      f"{median(sc) / rows:.3f} s per caption")
         if args.json:
             json.dump(res, open(args.json, "w"), indent=1)
         return

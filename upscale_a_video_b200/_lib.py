@@ -1,4 +1,4 @@
-"""ctypes binding of libuav_b200.so (the C ABI declared in include/uav_b200.h).
+"""ctypes binding of libuav_b200.so (the C ABI declared in include/uav_b200.h and include/uav_b200_int8.h).
 
 There is deliberately NO fallback: if the shared object is missing or a call fails, a
 RuntimeError is raised (SURVEY.md §8b "Errors": non-zero status -> Python raises).
@@ -116,6 +116,12 @@ _PROTOS = {
     "uav_attention_decode_batched": [P, I64, P, P, I64, I64, I64, I64, I32, I32, F32, P, I64, P, C.c_size_t, P],
     "uav_sample_top_p_batched": [P, I64, I64, I64, F32, F32, P, P, P],
 }
+# include/uav_b200_int8.h: the weight-only int8 decoder Linears of the LLaVA captioner (all int status)
+_INT8_PROTOS = {
+    "uav_quantize_rows_int8": [P, I64, I64, I64, P, P, P],
+    "uav_dequantize_rows_int8": [P, P, I64, I64, P, P],
+    "uav_gemv_rows_int8": [P, P, I64, I64, P, I64, P, P, I32, P],
+}
 _SPECIAL = {
     "uav_version": (C.c_char_p, []),
     "uav_last_error_string": (C.c_char_p, []),
@@ -134,7 +140,13 @@ def lib_path() -> Path:
 
 
 def declared_symbols():
+    """the symbols of include/uav_b200.h"""
     return list(_PROTOS) + list(_SPECIAL)
+
+
+def declared_int8_symbols():
+    """the symbols of include/uav_b200_int8.h"""
+    return list(_INT8_PROTOS)
 
 
 def load():
@@ -147,7 +159,7 @@ def load():
             "(nvcc, sm_90a). There is no CPU / PyTorch fallback for the sampling path."
         )
     lib = C.CDLL(str(_LIB_PATH))
-    for name, argtypes in _PROTOS.items():
+    for name, argtypes in (*_PROTOS.items(), *_INT8_PROTOS.items()):
         fn = getattr(lib, name)
         fn.argtypes = argtypes
         fn.restype = C.c_int

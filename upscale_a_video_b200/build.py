@@ -2,7 +2,8 @@
 
 `python -m upscale_a_video_b200.build` or `build()`; the resulting shared object lives in
 `upscale_a_video_b200/lib/` (git-ignored: a clean checkout builds it).
-No torch headers are involved: the library is a plain C-ABI CUDA library (include/uav_b200.h).
+No torch headers are involved: the library is a plain C-ABI CUDA library (include/uav_b200.h and
+include/uav_b200_int8.h).
 """
 from __future__ import annotations
 
@@ -40,7 +41,7 @@ def _sources():
 
 def _digest() -> str:
     h = hashlib.sha256()
-    for f in sorted(list(CSRC.glob("*.cu")) + list(CSRC.glob("*.cuh")) + [REPO / "include" / "uav_b200.h"]):
+    for f in sorted(list(CSRC.glob("*.cu")) + list(CSRC.glob("*.cuh")) + sorted((REPO / "include").glob("*.h"))):
         h.update(f.name.encode())
         h.update(f.read_bytes())
     h.update(" ".join(NVCC_FLAGS).encode())

@@ -17,6 +17,7 @@ upscale, with the reference's preprocessing and a generator seeded from SEED; th
 clip i is reached and has no caption yet, the first frames of clips i .. i + CAPTION_BATCH - 1 are captioned in one
 call, each with its own generator seeded SEED, which gives each clip the caption a call on it alone gives.  Under
 `torchrun` only rank 0 loads and runs the captioner and the captions are broadcast to the other ranks.
+`--llava_int8` loads the captioner with weight-only int8 decoder and projector Linears (`weights="int8"`).
 
 Deliberate differences from the reference CLI (INTEGRATION.md §3): the captioner runs only when `--llava_path` names a
 LLaVA-1.5 folder (otherwise `--caption` supplies the caption text), its sampling is seeded, errors raise instead of
@@ -63,11 +64,14 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--color_fix", type=str, default="None", choices=["None", "AdaIn", "Wavelet"])
     p.add_argument("--no_llava", action="store_true", default=False, help="Do not caption, even with --llava_path.")
     p.add_argument("--load_8bit_llava", action="store_true", default=False,
-                   help="Not supported: the captioner runs in fp16.")
+                   help="Not supported (bitsandbytes' LLM.int8()); see --llava_int8.")
     p.add_argument("--llava_path", type=str, default=None,
                    help="LLaVA-1.5 folder (released format): caption frame 0 of each clip with it.")
     p.add_argument("--llava_vision_path", type=str, default=None,
                    help="CLIP ViT-L/14-336 folder of the captioner's vision tower (default: the config's mm_vision_tower).")
+    p.add_argument("--llava_int8", action="store_true", default=False,
+                   help="Hold the captioner's decoder and projector Linears as weight-only int8 (about half the memory "
+                        "of fp16, and half the bytes per decoded token).")
     p.add_argument("--perform_tile", action="store_true", default=False)
     p.add_argument("--tile_size", type=int, default=256)
     p.add_argument("--save_image", action="store_true", default=False)
@@ -83,7 +87,10 @@ def parse_args(argv: Optional[List[str]] = None) -> argparse.Namespace:
     parser = build_parser()
     args = parser.parse_args(argv)
     if args.load_8bit_llava:
-        parser.error("--load_8bit_llava: there is no LLaVA captioner for 8-bit weights; it runs in fp16")
+        parser.error("--load_8bit_llava: there is no LLaVA captioner for bitsandbytes' LLM.int8() (int8 activations); "
+                     "--llava_int8 runs it on weight-only int8 Linears")
+    if args.llava_int8 and not use_llava(args):
+        parser.error("--llava_int8 needs the captioner: pass --llava_path (without --no_llava)")
     if args.caption and use_llava(args):
         parser.error("--caption and --llava_path both give the caption: pass one of them (or --no_llava)")
     return args
@@ -242,7 +249,8 @@ def main(argv: Optional[List[str]] = None) -> List[str]:
         if use_llava(args) and rank == 0:
             from .llava import LLavaAgent
             log("Loading LLaVA")
-            agent = LLavaAgent(args.llava_path, device=device, vision_tower_path=args.llava_vision_path)
+            agent = LLavaAgent(args.llava_path, device=device, vision_tower_path=args.llava_vision_path,
+                               weights="int8" if args.llava_int8 else "fp16")
         from .llava import CAPTION_BATCH
         captions: List[str] = []  # captions of the next clips, computed a group ahead
         written = []

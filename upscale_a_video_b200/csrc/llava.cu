@@ -131,14 +131,6 @@ constexpr int GEMV_MAX_K = 16384;
 constexpr int GEMV_MAX_ROWS = 8;
 constexpr int GEMV_ROWS_MAX_X = 8 * 13824;  // rows * K of x held in shared memory (216 KB: 8 rows of Llama-13B's down)
 
-__device__ __forceinline__ uint4 ldg16_stream(const void* p) {
-  uint4 r;
-  asm volatile("ld.global.nc.L1::no_allocate.L2::256B.v4.u32 {%0, %1, %2, %3}, [%4];"
-               : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w)
-               : "l"(p));
-  return r;
-}
-
 // acc[r] += w . x[r] over one 16-byte chunk (8 halves) for each input row r, in element order
 template <int ROWS>
 __device__ __forceinline__ void dot8_rows(const uint4& w, const uint4* __restrict__ sx, int chunks, float (&acc)[ROWS]) {

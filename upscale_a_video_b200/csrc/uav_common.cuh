@@ -352,6 +352,14 @@ __device__ __forceinline__ uint4 ldg16(const void* p) {
 __device__ __forceinline__ void stg16(void* p, const uint4& v) {
   *reinterpret_cast<uint4*>(p) = v;
 }
+// 16-byte streaming load of data read once (weight streams): non-coherent, no L1 allocation, 256-byte L2 prefetch
+__device__ __forceinline__ uint4 ldg16_stream(const void* p) {
+  uint4 r;
+  asm volatile("ld.global.nc.L1::no_allocate.L2::256B.v4.u32 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w)
+               : "l"(p));
+  return r;
+}
 
 // fp32 pair -> packed fp16, round to nearest
 __device__ __forceinline__ uint32_t pack_half2_rn(float a, float b) {

@@ -4,7 +4,9 @@
 The model folder is a LLaVA-1.5 release (`config.json`, `pytorch_model-*.bin` or `*.safetensors` shards with their index,
 the Llama sentencepiece `tokenizer.model`); the vision tower is a CLIP folder (`vision_model.*` of `pytorch_model.bin`
 or `model.safetensors`, and `preprocessor_config.json`).  Every weight is held once on the GPU, in fp16: the fused
-q|k|v and gate|up matrices are filled shard by shard as the checkpoint is read.
+q|k|v and gate|up matrices are filled shard by shard as the checkpoint is read.  With `weights="int8"` the decoder and
+projector Linears are held as weight-only int8 instead (`Int8Rows`, quantized on the GPU as each tensor is read): the
+decode GEMV streams the int8 rows, and the prefill GEMMs read each matrix dequantized to fp16 into one shared scratch.
 
 Path of one caption:
 - frame preprocessing on the host (`frame0_image`, `clip_preprocess`): the reference CLI's 512 bicubic resize, then
@@ -25,8 +27,9 @@ from __future__ import annotations
 
 import json
 import os
+import re
 from types import SimpleNamespace
-from typing import List, Optional
+from typing import List, NamedTuple, Optional
 
 import numpy as np
 import torch
@@ -36,7 +39,8 @@ from . import _lib, ops
 from .clip_text import encoder_layer
 
 __all__ = ["LLavaAgent", "IMAGE_TOKEN_INDEX", "conversation_prompt", "tokenize_prompt", "postprocess_caption",
-           "frame0_image", "clip_preprocess", "llava_key_map", "CAPTION_BATCH", "caption_groups"]
+           "frame0_image", "clip_preprocess", "llava_key_map", "CAPTION_BATCH", "caption_groups", "Int8Rows",
+           "WEIGHT_FORMATS"]
 
 IMAGE_TOKEN_INDEX = -200  # llava/constants.py
 DEFAULT_IMAGE_TOKEN = "<image>"
@@ -48,6 +52,7 @@ MAX_NEW_TOKENS = 64         # llava_agent.py: generate(max_new_tokens=64)
 FRAME_SHORT_SIDE = 512      # inference_upscale_a_video.py: fix_resize
 PATCH_K_PADDED = 592        # 3 * 14 * 14 = 588 patch values, padded to a multiple of 16 for the GEMM
 CAPTION_BATCH = 8           # images per weight pass: the batched GEMV and sampler take up to 8 rows
+WEIGHT_FORMATS = ("fp16", "int8")
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -165,6 +170,20 @@ def llava_key_map(cfg: SimpleNamespace) -> dict:
     return m
 
 
+class Int8Rows(NamedTuple):
+    """a weight-only int8 Linear (include/uav_b200_int8.h): int8 q (N, K) and the fp32 per-row absmax (N,) of the fp16
+    weight it was quantized from.  Decode computes with q * absmax / 127 exactly; the prefill with
+    fp16((q * absmax) / 127), one more rounding of at most 2^-12 relative per weight."""
+    q: torch.Tensor
+    absmax: torch.Tensor
+
+
+def _int8_linear(name: str) -> bool:
+    """the matrices held as int8 under weights="int8": every decoder Linear and the two projector Linears (as
+    transformers' load_in_8bit converts them); embed_tokens, lm_head and the RMSNorm weights stay fp16"""
+    return re.fullmatch(r"(qkv|o|gu|down)\d+|proj[02]_w", name) is not None
+
+
 def _decoder_shapes(cfg: SimpleNamespace) -> dict:
     H, I, V, Hv = cfg.hidden_size, cfg.intermediate_size, cfg.vocab_size, cfg.mm_hidden_size
     s = {"embed": ((V, H), torch.float16), "norm": ((H,), torch.float16), "lm_head": ((V, H), torch.float16),
@@ -177,11 +196,26 @@ def _decoder_shapes(cfg: SimpleNamespace) -> dict:
     return s
 
 
-def load_decoder(folder: str, cfg: SimpleNamespace, device) -> dict:
+def _quantize_into(t: torch.Tensor, dst: Int8Rows, device):
+    """quantizes the released tensor t (host) into dst on the device; its fp16 copy there is freed on return"""
+    ops.quantize_rows_int8(t.to(device=device, dtype=torch.float16), dst.q, dst.absmax)
+
+
+def load_decoder(folder: str, cfg: SimpleNamespace, device, weights: str = "fp16") -> dict:
     """the decoder and projector weights of a released LLaVA-1.5 folder, each held once on `device`.  Keys other than
-    the expected ones (`rotary_emb.inv_freq` buffers aside) and missing keys are errors."""
+    the expected ones (`rotary_emb.inv_freq` buffers aside) and missing keys are errors.  weights="int8" holds the
+    Linears of `_int8_linear` as `Int8Rows`, each released tensor quantized on the device as it is read: no fp16 copy
+    of the decoder is held, only one released tensor at a time."""
+    if weights not in WEIGHT_FORMATS:
+        raise ValueError(f"weights={weights!r}: one of {WEIGHT_FORMATS}")
     keymap, shapes = llava_key_map(cfg), _decoder_shapes(cfg)
-    out = {name: torch.empty(shape, dtype=dt, device=device) for name, (shape, dt) in shapes.items()}
+    out = {}
+    for name, (shape, dt) in shapes.items():
+        if weights == "int8" and _int8_linear(name):
+            out[name] = Int8Rows(torch.empty(shape, dtype=torch.int8, device=device),
+                                 torch.empty(shape[0], dtype=torch.float32, device=device))
+        else:
+            out[name] = torch.empty(shape, dtype=dt, device=device)
     filled = set()
     unexpected = []
     for k, t in _iter_tensors(_shard_files(folder)):
@@ -191,6 +225,13 @@ def load_decoder(folder: str, cfg: SimpleNamespace, device) -> dict:
             continue
         name, row = keymap[k]
         dst = out[name]
+        if isinstance(dst, Int8Rows):
+            dst = Int8Rows(dst.q[row:row + t.shape[0]], dst.absmax[row:row + t.shape[0]])
+            if tuple(dst.q.shape) != tuple(t.shape):
+                raise RuntimeError(f"{k}: shape {tuple(t.shape)} does not fit {tuple(dst.q.shape)}")
+            _quantize_into(t, dst, device)
+            filled.add(k)
+            continue
         if dst.dim() == 2:
             dst = dst[row:row + t.shape[0]]
         if tuple(dst.shape) != tuple(t.shape):
@@ -203,6 +244,13 @@ def load_decoder(folder: str, cfg: SimpleNamespace, device) -> dict:
     if missing:
         raise RuntimeError(f"missing keys in the LLaVA checkpoint: {missing[:5]}")
     return out
+
+
+def dequant_scratch(w: dict, device) -> Optional[torch.Tensor]:
+    """the fp16 buffer into which the prefill dequantizes each `Int8Rows` of w, sized for the largest (gate|up); None
+    when w holds none"""
+    n = max((t.q.numel() for t in w.values() if isinstance(t, Int8Rows)), default=0)
+    return torch.empty(n, dtype=torch.float16, device=device) if n else None
 
 
 def load_vision_tower(folder: str, vcfg: SimpleNamespace, layers: int, device) -> SimpleNamespace:
@@ -268,13 +316,20 @@ def _caption_generators(n: int, temperature: float, generator):
 # the agent
 # ---------------------------------------------------------------------------------------------------------------
 class LLavaAgent:
-    """`llava.llava_agent.LLavaAgent` on the uav_b200 kernels: fp16 weights, greedy decoding at temperature 0, top-p
-    sampling otherwise, with the uniforms drawn from `generator` (the global RNG when None)"""
+    """`llava.llava_agent.LLavaAgent` on the uav_b200 kernels: fp16 weights (or weight-only int8 decoder and projector
+    Linears with weights="int8"), greedy decoding at temperature 0, top-p sampling otherwise, with the uniforms drawn
+    from `generator` (the global RNG when None)"""
+    _dq = None  # the prefill's dequantization scratch (weights="int8")
 
     def __init__(self, model_path, device="cuda", conv_mode="vicuna_v1", load_8bit=False, load_4bit=False, *,
-                 vision_tower_path=None):
-        if load_8bit or load_4bit:
-            raise NotImplementedError("LLavaAgent runs in fp16: 8-bit and 4-bit loading are not supported")
+                 vision_tower_path=None, weights="fp16"):
+        if weights not in WEIGHT_FORMATS:
+            raise ValueError(f"weights={weights!r}: one of {WEIGHT_FORMATS}")
+        if load_8bit:
+            raise NotImplementedError("load_8bit (bitsandbytes' LLM.int8(): int8 activations with fp16 outlier columns) "
+                                      "is not supported; weights='int8' runs weight-only int8 decoder Linears")
+        if load_4bit:
+            raise NotImplementedError("4-bit loading is not supported (weights='fp16' or 'int8')")
         if conv_mode != "vicuna_v1":
             raise NotImplementedError(f"conv_mode {conv_mode!r}: only 'vicuna_v1' (LLaVA-1.5) is supported")
         model_path = os.path.expanduser(model_path)
@@ -338,7 +393,9 @@ class LLavaAgent:
             raise ValueError(f"mm_vision_select_layer {sel} out of range for {vc.num_hidden_layers} layers")
         with torch.cuda.device(self.device):
             self.tower = load_vision_tower(vt, vc, self.vision_layers, self.device)
-            self.w = load_decoder(model_path, cfg, self.device)
+            self.w = load_decoder(model_path, cfg, self.device, weights)
+            self._dq = dequant_scratch(self.w, self.device)
+        self.weights = weights
         self.qs = DEFAULT_QS
         self.conv_mode = conv_mode
         self.max_new_tokens = MAX_NEW_TOKENS
@@ -373,6 +430,20 @@ class LLavaAgent:
             x = encoder_layer(x, w, vc.num_attention_heads, vc.layer_norm_eps, act, causal=False)
         return x[0, 1:] if one else x[:, 1:]
 
+    def _prefill_weight(self, w):
+        """the fp16 weight a prefill GEMM reads: w itself, or an Int8Rows dequantized into the shared scratch.  The
+        scratch is overwritten by the next call; stream order runs the GEMM that reads it before that."""
+        if not isinstance(w, Int8Rows):
+            return w
+        return ops.dequantize_rows_int8(w.q, w.absmax, out=self._dq[:w.q.numel()].view(w.q.shape))
+
+    @staticmethod
+    def _gemv(w, x, **kw):
+        """the decode step's weight stream of w (fp16 or Int8Rows) over the rows x"""
+        if isinstance(w, Int8Rows):
+            return ops.gemv_rows_int8(w.q, w.absmax, x, **kw)
+        return ops.gemv_rows(w, x, **kw)
+
     # The layers take B sequences: x holds B x n prefill rows (sequence-major) or B decode rows, and the caches are
     # (B, L_max, hidden) (or (L_max, hidden) for B = 1).  The prefill GEMMs run on all B x n rows: uav_linear picks its
     # tile width from N alone for a single-tap GEMM without GEGLU, so each output element's k-order does not depend on
@@ -384,15 +455,15 @@ class LLavaAgent:
             kc, vc_ = kc[None], vc_[None]
         B = kc.shape[0]
         n = x.shape[0] // B
-        qkv = ops.linear(ops.rms_norm(x, w[f"ln1_{i}"], eps), w[f"qkv{i}"])
+        qkv = ops.linear(ops.rms_norm(x, w[f"ln1_{i}"], eps), self._prefill_weight(w[f"qkv{i}"]))
         ops.rope_kv_append_batched(qkv.view(B, n, -1), heads, 0, rope, kc, vc_)
         o = torch.empty(B * n, H, dtype=torch.float16, device=x.device)
         for b in range(B):  # the causal kernel reads a batch's keys n rows apart; each cache is L_max rows long
             ops.attention_causal(qkv[b * n:(b + 1) * n, :H].unsqueeze(0), kc[b, :n].unsqueeze(0),
                                  vc_[b, :n].unsqueeze(0), heads, out=o[b * n:(b + 1) * n].unsqueeze(0))
-        x = ops.linear(o, w[f"o{i}"], residual=x)
-        gu = ops.linear(ops.rms_norm(x, w[f"ln2_{i}"], eps), w[f"gu{i}"])
-        return ops.linear(ops.swiglu(gu), w[f"down{i}"], residual=x)
+        x = ops.linear(o, self._prefill_weight(w[f"o{i}"]), residual=x)
+        gu = ops.linear(ops.rms_norm(x, w[f"ln2_{i}"], eps), self._prefill_weight(w[f"gu{i}"]))
+        return ops.linear(ops.swiglu(gu), self._prefill_weight(w[f"down{i}"]), residual=x)
 
     def _layer_decode(self, i, x, pos, kc, vc_, rope):
         cfg, w = self.config, self.w
@@ -400,12 +471,12 @@ class LLavaAgent:
         if kc.dim() == 2:
             kc, vc_ = kc[None], vc_[None]
         B = x.shape[0]
-        qkv = ops.gemv_rows(w[f"qkv{i}"], ops.rms_norm(x, w[f"ln1_{i}"], eps))
+        qkv = self._gemv(w[f"qkv{i}"], ops.rms_norm(x, w[f"ln1_{i}"], eps))
         ops.rope_kv_append_batched(qkv.view(B, 1, -1), heads, pos, rope, kc, vc_)
         o = ops.attention_decode_batched(qkv[:, :H], kc, vc_, pos + 1, heads)
-        x = ops.gemv_rows(w[f"o{i}"], o, residual=x)
-        gu = ops.gemv_rows(w[f"gu{i}"], ops.rms_norm(x, w[f"ln2_{i}"], eps))
-        return ops.gemv_rows(w[f"down{i}"], ops.swiglu(gu), residual=x)
+        x = self._gemv(w[f"o{i}"], o, residual=x)
+        gu = self._gemv(w[f"gu{i}"], ops.rms_norm(x, w[f"ln2_{i}"], eps))
+        return self._gemv(w[f"down{i}"], ops.swiglu(gu), residual=x)
 
     def _logits(self, x_rows):
         """fp32 (B, vocab) logits of the rows x_rows (B, hidden) (a strided row view allowed)"""
@@ -431,9 +502,10 @@ class LLavaAgent:
         x = torch.empty(B, len(ids) - 1 + n_img, H, dtype=torch.float16, device=self.device)
         x[:, :at] = tok[:at]
         x[:, at + n_img:] = tok[at:]
-        h = ops.linear(feats.reshape(B * n_img, -1), w["proj0_w"], w["proj0_b"], act=ops.ACT_GELU)
+        h = ops.linear(feats.reshape(B * n_img, -1), self._prefill_weight(w["proj0_w"]), w["proj0_b"], act=ops.ACT_GELU)
+        proj2 = self._prefill_weight(w["proj2_w"])
         for b in range(B):
-            ops.linear(h[b * n_img:(b + 1) * n_img], w["proj2_w"], w["proj2_b"], out=x[b, at:at + n_img])
+            ops.linear(h[b * n_img:(b + 1) * n_img], proj2, w["proj2_b"], out=x[b, at:at + n_img])
         return x[0] if one else x
 
     @torch.no_grad()

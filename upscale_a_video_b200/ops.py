@@ -1076,3 +1076,54 @@ def sample_top_p_batched(logits: torch.Tensor, temperature: float, top_p: float,
     _lib.check(_lib.load().uav_sample_top_p_batched(logits.data_ptr(), logits.stride(0), B, V, temperature, top_p, us,
                                                     out.data_ptr(), _stream()), "uav_sample_top_p_batched")
     return out
+
+
+# weight-only int8 decoder Linears (include/uav_b200_int8.h): q int8 (N, K) with an fp32 per-row absmax (N,)
+def quantize_rows_int8(w: torch.Tensor, q: torch.Tensor, absmax: torch.Tensor):
+    """q[n] = round_half_even((w[n] * 127) / absmax[n]), absmax[n] = max |w[n]| (bitsandbytes' row-wise rule) of fp16
+    w (N, K) (a row slice of a wider matrix allowed), into int8 q (N, K) and fp32 absmax (N,), which may be row slices
+    of a larger destination"""
+    assert w.is_cuda and w.dtype == torch.float16 and w.dim() == 2 and w.stride(1) == 1
+    N, K = w.shape
+    assert q.dtype == torch.int8 and q.shape == (N, K) and q.is_contiguous()
+    assert absmax.dtype == torch.float32 and absmax.shape == (N,) and absmax.is_contiguous()
+    with _timed("quantize_int8", 0.0, 2.0 * N * K + N * K + 4.0 * N, f"quantize_int8 N{N} K{K}"):
+        _lib.check(_lib.load().uav_quantize_rows_int8(w.data_ptr(), N, K, w.stride(0), q.data_ptr(), absmax.data_ptr(),
+                                                      _stream()), "uav_quantize_rows_int8")
+
+
+def dequantize_rows_int8(q: torch.Tensor, absmax: torch.Tensor, out=None) -> torch.Tensor:
+    """fp16((q * absmax[n]) / 127) of int8 q (N, K) -> fp16 (N, K), the prefill's weight"""
+    assert q.is_cuda and q.dtype == torch.int8 and q.dim() == 2 and q.is_contiguous()
+    N, K = q.shape
+    assert absmax.dtype == torch.float32 and absmax.shape == (N,) and absmax.is_contiguous()
+    if out is None:
+        out = torch.empty(N, K, dtype=torch.float16, device=q.device)
+    assert out.dtype == torch.float16 and out.shape == (N, K) and out.is_contiguous()
+    with _timed("dequantize_int8", 0.0, N * K + 4.0 * N + 2.0 * N * K, f"dequantize_int8 N{N} K{K}"):
+        _lib.check(_lib.load().uav_dequantize_rows_int8(q.data_ptr(), absmax.data_ptr(), N, K, out.data_ptr(),
+                                                        _stream()), "uav_dequantize_rows_int8")
+    return out
+
+
+def gemv_rows_int8(q: torch.Tensor, absmax: torch.Tensor, x: torch.Tensor, *, residual=None, out=None,
+                   out_dtype=torch.float16):
+    """out (rows, N) = (x (rows, K) @ q (N, K)^T) * absmax / 127 (+ residual (rows, N)), 1 <= rows <= 8, the int8
+    weight stream of a decode step; each row's result does not depend on the other rows"""
+    assert q.is_cuda and q.dtype == torch.int8 and q.dim() == 2 and q.is_contiguous()
+    N, K = q.shape
+    assert absmax.dtype == torch.float32 and absmax.shape == (N,) and absmax.is_contiguous()
+    assert x.dtype == torch.float16 and x.dim() == 2 and x.shape[1] == K and x.is_contiguous()
+    rows = x.shape[0]
+    assert 1 <= rows <= 8, rows
+    if out is None:
+        out = torch.empty(rows, N, dtype=out_dtype, device=q.device)
+    assert out.shape == (rows, N) and out.is_contiguous() and out.dtype in (torch.float16, torch.float32)
+    if residual is not None:
+        assert residual.dtype == torch.float16 and residual.shape == (rows, N) and residual.is_contiguous()
+    with _timed("gemv", 2.0 * rows * N * K, N * K + 4.0 * N + 2.0 * rows * (K + N), f"gemv_rows_int8 {rows} N{N} K{K}"):
+        _lib.check(_lib.load().uav_gemv_rows_int8(q.data_ptr(), absmax.data_ptr(), N, K, x.data_ptr(), rows,
+                                                  0 if residual is None else residual.data_ptr(), out.data_ptr(),
+                                                  F16 if out.dtype == torch.float16 else F32, _stream()),
+                   "uav_gemv_rows_int8")
+    return out
