@@ -135,6 +135,16 @@ struct alignas(64) IgemmParams {
   float out_scale;     // applied before the residual add (1 = off)
   float* gn_partial;   // [n_out / 8][gn_blocks][2] GroupNorm statistics of the output, or nullptr
   int64_t gn_blocks;
+  int32_t epi_kind;    // EPI_* feature set of a specialised AUX epilogue body, or EPI_GENERIC
+};
+
+// Feature sets of the AUX epilogue of the TMA-store instance that have a body of their own, compiled with only their
+// features (no activation, no GEGLU).  A residual is added as fmaf(x, out_scale, r) whatever out_scale is, so EPI_SCALE
+// only marks out_scale without a residual.  Every other combination runs the generic body (EPI_GENERIC).
+constexpr int EPI_ROWVEC = 1, EPI_RES = 2, EPI_STATS = 4, EPI_SCALE = 8, EPI_GENERIC = -1;
+template <int F>
+struct EpiKindTag {
+  static constexpr int value = F;
 };
 
 template <int BLOCK_N, bool GEGLU>
@@ -387,6 +397,19 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
     // each pass: an unrolled 256-column AUX epilogue would be twice the code and no longer fit the instruction cache.
     constexpr int EPI_N = GEGLU ? OUT_TILE_N : (OUT_TILE_N < 128 ? OUT_TILE_N : 128);
     constexpr int EPI_ACC = EPI_N / 2;
+    // GroupNorm statistics of one pass: stats[2 jb], stats[2 jb + 1] = {sum, sum of squares} of column group jb over the
+    // thread's rows; the warp's 16 rows x 8 columns per group are one block
+    auto store_stats = [&](auto& stats, int pass) {
+      // lane l ends up with the warp's sum of stats[l >> SHIFT]
+      constexpr int SHIFT = EPI_N == 128 ? 0 : 1;
+      static_assert(!TMA_EPI || EPI_N / 4 == (32 >> SHIFT), "one statistics value per 2^SHIFT lanes");
+      const float s = warp_sum_transpose(stats, lane);
+      const int value = lane >> SHIFT;
+      const int oct = ((n_base + pass * EPI_N) >> 3) + (value >> 1);
+      const int64_t blk = static_cast<int64_t>(tile.m_tile) * 8 + cw;
+      if ((lane & ((1 << SHIFT) - 1)) == 0 && blk < p.gn_blocks && oct * 8 < p.n_out)
+        p.gn_partial[(static_cast<int64_t>(oct) * p.gn_blocks + blk) * 2 + (value & 1)] = s;
+    };
     auto epilogue = [&](auto act_tag) {
       [[maybe_unused]] constexpr int ACT = decltype(act_tag)::value;
 #pragma unroll 1
@@ -467,18 +490,81 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
           }
         }
         if constexpr (AUX && TMA_EPI) {
-          if (p.gn_partial != nullptr) {  // warp-uniform: the 16 rows x 8 columns of this warp per column group
-            // lane l ends up with the warp's sum of stats[l >> SHIFT]
-            constexpr int SHIFT = EPI_N == 128 ? 0 : 1;
-            static_assert(EPI_N / 4 == (32 >> SHIFT), "one statistics value per 2^SHIFT lanes");
-            const float s = warp_sum_transpose(stats, lane);
-            const int value = lane >> SHIFT;
-            const int oct = ((n_base + pass * EPI_N) >> 3) + (value >> 1);
-            const int64_t blk = static_cast<int64_t>(tile.m_tile) * 8 + cw;
-            if ((lane & ((1 << SHIFT) - 1)) == 0 && blk < p.gn_blocks && oct * 8 < p.n_out)
-              p.gn_partial[(static_cast<int64_t>(oct) * p.gn_blocks + blk) * 2 + (value & 1)] = s;
+          if (p.gn_partial != nullptr) store_stats(stats, pass);  // warp-uniform
+        }
+        if (pass + 1 < OUT_TILE_N / EPI_N) {
+#pragma unroll
+          for (int i = 0; i + EPI_ACC < Cfg::ACC; ++i) acc[i] = acc[i + EPI_ACC];
+        }
+      }
+    };
+    // The AUX body of one feature set (EPI_*) of the TMA-store epilogue without activation.  It makes each of the generic
+    // body's run-time decisions once per tile or once per 8-column group instead of once per element pair, and keeps its
+    // fp32 operations and their order: (acc + bias) + rowvec, fmaf(x, out_scale, residual) or x * out_scale, statistics,
+    // saturating fp16, so outputs and statistics are bitwise the generic body's.
+    auto epilogue_kind = [&](auto kind_tag) {
+      constexpr int F = decltype(kind_tag)::value;
+      constexpr bool ROWVEC = (F & EPI_ROWVEC) != 0, RES = (F & EPI_RES) != 0, STATS = (F & EPI_STATS) != 0,
+                     SCALE = (F & EPI_SCALE) != 0;
+      const bool has_bias = p.bias != nullptr;  // float2 loads: the host checked 8-byte alignment
+      // row vectors of the thread's two rows; a row outside the output takes the other row's (its value is never
+      // stored or counted), and when both rows share one, it is loaded once per column group
+      [[maybe_unused]] const __half* rvp[2];
+      [[maybe_unused]] bool rv_shared = true;
+      if constexpr (ROWVEC) {
+        rvp[0] = rv[0] != nullptr ? rv[0] : (rv[1] != nullptr ? rv[1] : p.rowvec);
+        rvp[1] = rv[1] != nullptr ? rv[1] : rvp[0];
+        rv_shared = rvp[0] == rvp[1];
+      }
+#pragma unroll 1
+      for (int pass = 0; pass < OUT_TILE_N / EPI_N; ++pass) {
+        [[maybe_unused]] float stats[EPI_N / 4];
+#pragma unroll
+        for (int jb = 0; jb < EPI_N / 8; ++jb) {
+          const int col = pass * EPI_N + jb * 8 + 2 * lr;
+          const int n = n_base + col;
+          float gs = 0.f, gq = 0.f;
+          // n_out % 8 == 0 on the TMA-store path: a group of 8 columns is wholly inside or wholly outside the output
+          if (n_base + pass * EPI_N + jb * 8 < p.n_out) {
+            float2 b = make_float2(0.f, 0.f);
+            if (has_bias) b = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+            [[maybe_unused]] float2 rvf[2];
+            if constexpr (ROWVEC) {
+              rvf[0] = __half22float2(__ldg(reinterpret_cast<const __half2*>(rvp[0] + n)));
+              rvf[1] = rv_shared ? rvf[0] : __half22float2(__ldg(reinterpret_cast<const __half2*>(rvp[1] + n)));
+            }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              float x0 = acc[4 * jb + 2 * h] + b.x, x1 = acc[4 * jb + 2 * h + 1] + b.y;
+              const uint32_t row = lrow[h];
+              uint8_t* sp = staging + (col >> 6) * SLAB_BYTES + row * 128 + ((((col & 63) >> 3) ^ (row & 7)) << 4) + (col & 7) * 2;
+              if constexpr (ROWVEC) {
+                x0 += rvf[h].x;
+                x1 += rvf[h].y;
+              }
+              if constexpr (RES) {
+                const float2 r = __half22float2(*reinterpret_cast<const __half2*>(sp));
+                x0 = fmaf(x0, p.out_scale, r.x);
+                x1 = fmaf(x1, p.out_scale, r.y);
+              } else if constexpr (SCALE) {
+                x0 *= p.out_scale;
+                x1 *= p.out_scale;
+              }
+              if constexpr (STATS) {
+                if (row_ok[h]) {
+                  gs += x0 + x1;
+                  gq = fmaf(x0, x0, fmaf(x1, x1, gq));
+                }
+              }
+              *reinterpret_cast<uint32_t*>(sp) = pack_half2_sat(x0, x1);
+            }
+          }
+          if constexpr (STATS) {
+            stats[2 * jb] = gs;
+            stats[2 * jb + 1] = gq;
           }
         }
+        if constexpr (STATS) store_stats(stats, pass);
         if (pass + 1 < OUT_TILE_N / EPI_N) {
 #pragma unroll
           for (int i = 0; i + EPI_ACC < Cfg::ACC; ++i) acc[i] = acc[i + EPI_ACC];
@@ -487,11 +573,24 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
     };
     // The activation is the same for the whole launch, so it is picked here, once per tile, and each epilogue body is
     // compiled for one activation: the run-time switch inlined at every element pair made the AUX epilogue several
-    // times as long as the one without activation, and launches without one or with SiLU pay for none of it.
-    if constexpr (AUX) {
+    // times as long as the one without activation, and launches without one or with SiLU pay for none of it.  The
+    // feature sets the UNet and the VAE launch have bodies of their own, picked the same way.
+    auto epilogue_generic = [&] {
       if (p.act == UAV_ACT_SILU) epilogue(ActTag<UAV_ACT_SILU>{});
       else if (p.act == UAV_ACT_NONE || p.act == UAV_ACT_GEGLU) epilogue(ActTag<UAV_ACT_NONE>{});
       else epilogue(ActTag<ACT_RUNTIME>{});
+    };
+    if constexpr (AUX && TMA_EPI && !GEGLU) {
+      switch (p.epi_kind) {
+        case EPI_ROWVEC | EPI_STATS: epilogue_kind(EpiKindTag<EPI_ROWVEC | EPI_STATS>{}); break;
+        case EPI_RES | EPI_STATS: epilogue_kind(EpiKindTag<EPI_RES | EPI_STATS>{}); break;
+        case EPI_RES: epilogue_kind(EpiKindTag<EPI_RES>{}); break;
+        case EPI_STATS: epilogue_kind(EpiKindTag<EPI_STATS>{}); break;
+        case EPI_SCALE: epilogue_kind(EpiKindTag<EPI_SCALE>{}); break;
+        default: epilogue_generic();
+      }
+    } else if constexpr (AUX) {
+      epilogue_generic();
     } else {
       epilogue(ActTag<UAV_ACT_NONE>{});
     }
@@ -541,6 +640,14 @@ static uav_status_t launch_instance(IgemmParams& p, cudaStream_t stream) {
   const dim3 grid(p.num_tiles < sms ? p.num_tiles : sms);
   const bool aux = p.rowvec != nullptr || p.residual != nullptr || (p.act != UAV_ACT_NONE && p.act != UAV_ACT_GEGLU) ||
                    p.out_scale != 1.0f || p.gn_partial != nullptr;
+  p.epi_kind = EPI_GENERIC;
+  if (p.tma_store && !GEGLU && p.act == UAV_ACT_NONE && (reinterpret_cast<uintptr_t>(p.bias) & 7) == 0) {
+    const int kind = (p.rowvec != nullptr ? EPI_ROWVEC : 0) | (p.res_tma ? EPI_RES : 0) |
+                     (p.gn_partial != nullptr ? EPI_STATS : 0) |
+                     (p.residual == nullptr && p.out_scale != 1.0f ? EPI_SCALE : 0);
+    for (int k : {EPI_ROWVEC | EPI_STATS, EPI_RES | EPI_STATS, EPI_RES, EPI_STATS, EPI_SCALE})
+      if (kind == k) p.epi_kind = kind;
+  }
   if constexpr (Cfg::OUT_TILE_N >= 64) {
     if (p.tma_store) {
       return aux ? launch_opted_in<igemm_kernel<BLOCK_N, GEGLU, true, true>>(grid, NUM_THREADS, smem, stream, p)
